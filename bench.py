@@ -1,11 +1,12 @@
 #!/usr/bin/env python
-"""bench.py -- the hot-path benchmark (contract: see the task statement / DESIGN.md section 6).
+"""bench.py -- the hot-path benchmark (one JSON result line per run).
 
-Metric (BASELINE.json): GP log_probability/sec at N=65536, dense ExpSquared 3-D, fp64.
+Metric: GP log_probability/sec at N=65536, dense ExpSquared 3-D, fp64.
 A "step" is one full ``log_probability``: kernel-matrix build fused into the blocked Cholesky,
 forward triangular solve, log-determinant and |alpha|^2 reductions.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload dense|quasisep]
+                  [--dump-outputs DIR]
 
 * ``value``  : device-timed throughput with X / diag / y already resident in HBM.
 * ``e2e``    : the same metric through the public API ``GaussianProcess(kernel, X, diag=...).log_probability(y)``
@@ -13,6 +14,9 @@ forward triangular solve, log-determinant and |alpha|^2 reductions.
 * ``roofline``: trailing-update DMMA kernel, algorithmic flop / summed CUDA-event time of its launches,
                against the fp64 tensor (DMMA) peak measured by our own micro-benchmark on this GPU
                (MEASURED_PEAKS.json carries only bf16/HBM peaks; fp64 has no entry there).
+* ``--dump-outputs DIR``: after the timed steps, what the timed path returned in its last step (the log-probability,
+               plus the per-problem values of the batched workload) as DIR/<name>.npy in float64.  The inputs are seeded,
+               so two builds can be compared output for output.
 * ``cpu_baseline`` / ``--impl reference``: the NumPy/SciPy oracle port (the reference needs JAX, which is not
                installed here or on the box) on the host cores, on a bounded sample, extrapolated as stated.
 N > 1: one process per GPU; the dense path runs as independent replicas (one hyper-parameter point per
@@ -41,7 +45,7 @@ SEED = 49382
 
 
 def make_dense_problem(n, rank=0):
-    """SURVEY 8(d) C2: X ~ U(0,20)^3 at N=65536 (same point density for other N), y = sin(x0) + 0.1 N(0,1),
+    """X ~ U(0,20)^3 at N=65536 (same point density for other N), y = sin(x0) + 0.1 N(0,1),
     1.0 * ExpSquared(scale=1.0), diag=0.1.  Ranks > 0 evaluate a neighbouring length scale."""
     rng = np.random.default_rng(SEED)
     side = 20.0 * (n / 65536.0) ** (1.0 / 3.0)
@@ -50,6 +54,19 @@ def make_dense_problem(n, rank=0):
     diag = np.full(n, 0.1)
     scale = 1.0 + 0.01 * rank
     return X, y, diag, scale
+
+
+def dump_outputs(directory, arrays):
+    """DIR/<name>.npy (float64) for each array; at most 64 MB in all"""
+    if not directory:
+        return
+    os.makedirs(directory, exist_ok=True)
+    total = 0
+    for name, a in arrays.items():
+        a = np.atleast_1d(np.asarray(a, dtype=np.float64))
+        total += a.nbytes
+        assert total <= 64 << 20, "dumped outputs exceed 64 MB"
+        np.save(os.path.join(directory, f"{name}.npy"), a)
 
 
 def golden_check(which, n, logp):
@@ -66,7 +83,7 @@ def golden_check(which, n, logp):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -233,7 +250,7 @@ def run_ours(args, rank, local_rank, world):
     from tinygp_b200 import GaussianProcess, _cabi, kernels
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device visible; the B200 solver has no CPU fallback")
+        raise SystemExit("bench.py: no CUDA device visible; the solver has no CPU fallback")
     torch.cuda.set_device(local_rank)
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
@@ -312,6 +329,8 @@ def run_ours(args, rank, local_rank, world):
         sampler.start()
     ms, logp = timed(step_device, args.steps, per_step_ms)
     clocks = sampler.stop() if rank == 0 else None
+    if rank == 0:
+        dump_outputs(args.dump_outputs, {"dense_logp": logp})
     prof = ctx.profile(reset=True)
     ctx.set_option("profile", 0)
     launches = ctx.launch_count() - l0
@@ -339,6 +358,7 @@ def run_ours(args, rank, local_rank, world):
                 try:
                     ctx.reset_options()
                     sub_records[name] = fn(args, ctx, local_rank)
+                    sub_records[name].pop("logp_all", None)
                 except Exception as e:  # noqa: BLE001
                     sub_records[name] = {"error": str(e)[:300]}
                 ctx.set_option("trim", 0)
@@ -359,16 +379,15 @@ def run_ours(args, rank, local_rank, world):
         except Exception:
             bf16 = {}
         roofline = {
-            "bound": "tensor", "kernel": "i8_update_kernel (tcgen05.mma kind::i8, TMA multicast, TMEM int32 accumulators)",
+            "bound": "tensor", "kernel": "i8_update_kernel (wgmma s8 x s8 -> s32, TMA multicast, register accumulators)",
             "achieved": i8_tops, "peak": i8_peak_sustained, "unit": "TFLOP/s", "frac": i8_tops / i8_peak_sustained,
             "peak_source": "int8 tensor TOP/s measured on this GPU by b200gp_measure_i8_peak (resident-operand "
-                           "tcgen05 loop, ~1 s); MEASURED_PEAKS.json has bf16 only (int8 nominal = 2x bf16)",
+                           "wgmma loop, ~1 s); MEASURED_PEAKS.json has bf16 only (int8 nominal = 2x bf16)",
             "peak_burst": i8_peak_burst, "bf16_measured_peaks": {k: bf16.get(k) for k in ("bf16_tflops", "bf16_tflops_sustained")},
             "int8_ops_per_step": prof["i8_ops"] / args.steps, "digit_planes": args.slices,
             "fp64_equivalent_tflops": syrk_tf, "fp64_dmma_peak_sustained": peak_sustained, "fp64_dmma_peak_burst": peak_burst,
             "launches": int(prof["syrk_launches"]), "ms_total": prof["syrk_ms"],
             "whole_step_tflops_n3_over_3": flop_alg * args.steps / (ms * 1e-3) / 1e12,
-            "traffic": _read_traffic(),
         }
     else:
       roofline = {
@@ -379,7 +398,6 @@ def run_ours(args, rank, local_rank, world):
         "peak_burst": peak_burst, "dfma_sustained": dfma_sustained,
         "launches": int(prof["syrk_launches"]), "ms_total": prof["syrk_ms"],
         "whole_step_tflops_n3_over_3": flop_alg * args.steps / (ms * 1e-3) / 1e12,
-        "traffic": _read_traffic(),
       }
     # CPU baseline on a bounded sample (rank 0 at N=1 only)
     if world == 1 and not args.quick:
@@ -399,11 +417,11 @@ def run_ours(args, rank, local_rank, world):
         "vs_baseline": None, "dtype": "f64", "data": "synthetic",
         "config": {"workload": f"dense ExpSquared 3-D N={n} log_probability (fused build + blocked Cholesky + solve)",
                    "kernel": "1.0*ExpSquared(scale=1.0), L2", "diag": 0.1, "seed": SEED, "nb": args.nb,
-                   "trailing_update": (f"int8 fixed-point, {args.slices} digit planes (tcgen05 kind::i8)" if args.slices
+                   "trailing_update": (f"int8 fixed-point, {args.slices} digit planes (wgmma s8)" if args.slices
                                        else "native fp64 DMMA"),
                    "options": args.opt, "quick": bool(args.quick),
                    "parallelism": f"replicas x{world}" if world > 1 else "single GPU",
-                   "l2": "working set 34 GB >> 126 MB L2 (no flush needed)"},
+                   "l2": "working set 34 GB >> 50 MB L2 (no flush needed)"},
         "logp": logp, "logp_e2e": logp_e2e, "golden": golden_check("c2", n, logp),
         "roofline": roofline, "cpu_baseline": cpu_baseline, "clocks": clocks,
         "e2e": {"value": e2e_value, "unit": "logp/s", "steps": e2e_steps,
@@ -431,10 +449,10 @@ def _hbm_peak():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"], "MEASURED_PEAKS.json hbm_gbs (measured)"
     except Exception:
-        return 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet: 3.35 TB/s HBM3 (not measured)"
 
 
-def measure_quasisep(args, ctx, local_rank, n=10_000_000, steps=None, warmup=3, opts=()):
+def measure_quasisep(args, ctx, local_rank, n=10_000_000, steps=None, warmup=3, opts=(), exact_steps=False):
     """BASELINE config 4: SHO + Matern-3/2 (J = 4) on a sorted 1-D series of N = 1e7 points, one GPU.
     `value`: device-resident inputs through b200gp_qs_log_probability_dev; `e2e`: GaussianProcess(...).log_probability(y)
     with host buffers.  The C restatement of the sequential recursion (oracle/csrc) checks the FULL series."""
@@ -488,7 +506,8 @@ def measure_quasisep(args, ctx, local_rank, n=10_000_000, steps=None, warmup=3, 
     sampler = ClockSampler(local_rank)
     sampler.start()
     ms_cal, _ = timed(step_device, 10)
-    reps = max(steps, int(2000.0 / max(ms_cal / 10.0, 1e-3)))   # a step is ~1 ms: ~2 s of them so that nvidia-smi samples the clocks
+    # a step is ~1 ms: as a sub-record, ~2 s of them so that nvidia-smi samples the clocks; as the workload, exactly --steps
+    reps = steps if exact_steps else max(steps, int(2000.0 / max(ms_cal / 10.0, 1e-3)))
     ctx.profile(reset=True)
     l0 = ctx.launch_count()
     ms, logp = timed(step_device, reps)
@@ -500,7 +519,7 @@ def measure_quasisep(args, ctx, local_rank, n=10_000_000, steps=None, warmup=3, 
     e2e_steps = 2
     ms_e2e, logp_e2e = timed(step_e2e, e2e_steps)
     J = kernel.state_dim()
-    alg_bytes = 8.0 * n * (3 + 1 + J)          # read t, diag, y ; write c, w   (SURVEY 8d: 64 B/point at J=4)
+    alg_bytes = 8.0 * n * (3 + 1 + J)          # read t, diag, y ; write c, w   (64 B/point at J=4)
     hbm_peak, src = _hbm_peak()
     achieved = alg_bytes * reps / (prof["qs_ms"] * 1e-3) / 1e9
     # parity at FULL size: the C restatement of ops.py:352-365,463-472 on all N points (1 core)
@@ -515,14 +534,14 @@ def measure_quasisep(args, ctx, local_rank, n=10_000_000, steps=None, warmup=3, 
         "metric": "log_probability/sec", "value": reps / (ms * 1e-3), "unit": "logp/s", "n_gpus": 1,
         "steps": reps, "warmup": warmup, "ms_per_step": ms / reps, "higher_is_better": True, "dtype": "f64", "data": "synthetic",
         "config": {"workload": f"quasisep SHO+Matern32 (J=4) N={n} log_probability", "diag": 0.1, "seed": 49384,
-                   "options": list(opts), "l2": "working set 0.64 GB > 126 MB L2"},
+                   "options": list(opts), "l2": "working set 0.64 GB > 50 MB L2"},
         "logp": logp, "logp_e2e": logp_e2e,
         "parity": {"oracle_logp": lpo, "rel_err": abs(logp - lpo) / abs(lpo), "rel_err_e2e": abs(logp_e2e - lpo) / abs(lpo),
                    "oracle": f"C restatement of the sequential recursion on all {n} points ({t_cpu:.2f} s, 1 core)"},
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": hbm_peak, "unit": "GB/s", "frac": achieved / hbm_peak,
-                     "peak_source": src, "traffic": _read_traffic("qs_traffic.json", "dram_bytes_per_step") if n == 10_000_000 else None,
+                     "peak_source": src,
                      "algorithmic_bytes_per_point": 8 * (3 + 1 + J),
-                     "note": "fp64-ALU bound (Riccati composites + exp/sincos per point), see DESIGN.md section 4"},
+                     "note": "fp64-ALU bound (Riccati composites + exp/sincos per point)"},
         "cpu_baseline": {"value": 1.0 / t_cpu, "unit": "logp/s", "cores": 1, "kind": "port",
                          "sample": f"all {n} points, C restatement of ops.py:352-365,463-472 ({t_cpu:.2f} s; generators "
                                    f"precomputed with NumPy, not timed)"},
@@ -541,8 +560,9 @@ def run_quasisep(args, rank, local_rank, world):
     if args.qs_chunk:
         ctx.set_option("qs_chunk", args.qs_chunk)
     n = args.n if args.n != N_DENSE else 10_000_000
-    line = measure_quasisep(args, ctx, local_rank, n=n, steps=args.steps, warmup=args.warmup, opts=args.opt)
+    line = measure_quasisep(args, ctx, local_rank, n=n, steps=args.steps, warmup=args.warmup, opts=args.opt, exact_steps=True)
     line.update({"scaling": "weak", "vs_baseline": None})
+    dump_outputs(args.dump_outputs, {"quasisep_logp": line["logp"]})
     print(json.dumps(line), flush=True)
 
 
@@ -608,7 +628,7 @@ def measure_batched(args, ctx, local_rank, rank=0, world=1, n=4096, steps=2, war
         "roofline": {"bound": "tensor", "achieved": tf, "unit": "TFLOP/s", "peak": None,
                      "note": "native fp64 DMMA path (N = 4096 < ozaki_min_n); DMMA peak measured by the dense line"},
         "parity": {"max_rel_err_vs_oracle_on_grid_corners": max(checks) if checks else None},
-        "logp_first": float(out[0]), "clocks": clocks,
+        "logp_first": float(out[0]), "clocks": clocks, "logp_all": out.copy(),
     }
 
 
@@ -625,6 +645,8 @@ def run_batched(args, rank, local_rank, world):
         key, _, val = kv.partition("=")
         ctx.set_option(key, int(val))
     line = measure_batched(args, ctx, local_rank, rank, world, n=n, steps=args.steps, warmup=args.warmup)
+    if rank == 0:
+        dump_outputs(args.dump_outputs, {"batched_logp": line.pop("logp_all")})
     if args.opt:
         line["config"]["options"] = list(args.opt)
     if rank == 0:
@@ -633,10 +655,13 @@ def run_batched(args, rank, local_rank, world):
         dist.destroy_process_group()
 
 
-def measure_sharded(args, ctx, rank, local_rank, world, n=131072, steps=2, warmup=1, slices=None):
+N_SHARDED = 98304   # every rank holds all digit planes: 7 x N^2 bytes = 68 GB of an H100's 80 GB
+
+
+def measure_sharded(args, ctx, rank, local_rank, world, n=N_SHARDED, steps=2, warmup=1, slices=None):
     """BASELINE config 3: ONE dense log_probability sharded over the GPUs.  Kernel 1.5*Matern52(2.0) +
-    0.7*RationalQuadratic(1.5, alpha=1.5), both with the Euclidean metric (the L1 defaults are indefinite in 3-D, see
-    DESIGN.md section 2), N = 131072 by default.  Strong scaling.  Collective: every rank must call this."""
+    0.7*RationalQuadratic(1.5, alpha=1.5), both with the Euclidean metric (the L1 defaults are indefinite in 3-D),
+    N = N_SHARDED by default.  Strong scaling.  Collective: every rank must call this."""
     import torch
     import torch.distributed as dist
     from tinygp_b200 import kernels, multigpu
@@ -688,7 +713,7 @@ def measure_sharded(args, ctx, rank, local_rank, world, n=131072, steps=2, warmu
         "config": {"workload": f"dense Matern52+RationalQuadratic (L2) 3-D N={n}: ONE log_probability sharded over "
                                f"{world} GPU(s), int8 fixed-point update ({slices} digit planes)",
                    "diag": 0.1, "seed": 49383, "nb": args.nb, "exchange": stats.get("exchange", "all_gather_into_tensor per block column")},
-        "logp": lp, "golden": golden_check("c3", n, lp) or golden_check("c3s", n, lp),
+        "logp": lp, "golden": golden_check("c3s", n, lp) or "no stored known answer at this N (tests/golden/full_size.json has c3s, N = 65537)",
         "tflops_n3_over_3": n ** 3 / 3.0 * steps / t / 1e12,
         "kernel_ms_per_step_rank0": {"i8_update": prof["syrk_ms"] / steps, "panel": prof["panel_ms"] / steps,
                                      "build_cut": prof["build_ms"] / steps, "solve": prof["solve_ms"] / steps},
@@ -715,22 +740,13 @@ def run_sharded(args, rank, local_rank, world):
     for kv in args.opt:
         key, _, val = kv.partition("=")
         ctx.set_option(key, int(val))
-    n = 131072 if args.n == N_DENSE else args.n
+    n = N_SHARDED if args.n == N_DENSE else args.n
     line = measure_sharded(args, ctx, rank, local_rank, world, n=n, steps=args.steps, warmup=args.warmup)
     if rank == 0:
+        dump_outputs(args.dump_outputs, {"sharded_logp": line["logp"]})
         print(json.dumps(line), flush=True)
     if world > 1:
         dist.destroy_process_group()
-
-
-def _read_traffic(name="syrk_traffic.json", key="dram_bytes_per_launch"):
-    """DRAM read + write bytes of the dominant kernel(s) from the committed ncu capture (profiles/): per launch for the int8
-    update, per step for the two point-wise quasiseparable passes"""
-    p = os.path.join(ROOT, "profiles", name)
-    try:
-        return json.load(open(p)).get(key)
-    except Exception:
-        return None
 
 
 def main():
@@ -743,14 +759,15 @@ def main():
     ap.add_argument("--nb", type=int, default=1024)
     ap.add_argument("--qs-chunk", type=int, default=0)
     ap.add_argument("--workload", default="dense", choices=["dense", "quasisep", "batched", "sharded"])
-    ap.add_argument("--slices", type=int, default=7,
-                    help="int8 digit planes of the fixed-point trailing update: 7 = 48 bits under the row scale (default: "
-                         "same 4.7e-12 distance to the LAPACK golden at N=65536 as 8 planes), 8 = 55 bits, "
-                         "0 = native fp64 DMMA")
+    ap.add_argument("--slices", type=int, default=0,
+                    help="0 = native fp64 DMMA trailing update (default: the faster path on the H100); int8 digit planes of "
+                         "the fixed-point update: 7 = 48 bits under the row scale, 8 = 55 bits")
     ap.add_argument("--quick", action="store_true",
                     help="tuning sweeps: skip the e2e and cpu_baseline legs (the printed line is not a valid bench line)")
     ap.add_argument("--no-sub", action="store_true",
                     help="dense workload: skip the attached sub-records (C4 quasisep, C5 batched; sharded C3 when WORLD_SIZE > 1)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the timed path returned in its last step as DIR/<name>.npy")
     ap.add_argument("--opt", action="append", default=[], metavar="KEY=INT",
                     help="library option for tuning runs (b200gp_set_option); dense and quasisep workloads")
     args = ap.parse_args()

@@ -105,13 +105,11 @@ int b200gp_get_profile(b200gp_ctx* ctx, b200gp_profile* out, int reset);
 /* fp64 tensor (DMMA) peak micro-benchmark on this device: returns achieved TFLOP/s of a
  * register-resident mma.sync.m8n8k4.f64 loop on all SMs, and of a DFMA loop. */
 int b200gp_measure_fp64_peak(b200gp_ctx* ctx, double* dmma_tflops, double* dfma_tflops);
-/* int8 tensor peak micro-benchmark: tcgen05.mma kind::i8 (M=128, N=256, K=32) issued back to back on every SM
+/* int8 tensor peak micro-benchmark: wgmma.m64n128k32.s32.s8.s8 issued back to back by two warpgroups on every SM
  * from resident shared-memory operands (no TMA traffic); returns TOP/s (2 x MAC). */
 int b200gp_measure_i8_peak(b200gp_ctx* ctx, double* tops);
-/* same with tcgen05.mma.cta_group::2 on CTA pairs (M = 256) */
-int b200gp_measure_i8_peak_2sm(b200gp_ctx* ctx, double* tops);
 
-/* diagnostics for the int8 fixed-point tensor-core update (tcgen05.mma kind::i8, ozaki.cu):
+/* diagnostics for the int8 fixed-point tensor-core update (wgmma s8 x s8 -> s32, ozaki.cu):
  * C (rows x rows, host, in/out) -= sum_{s+t<S} 2^-(12+7(s+t)) rs_i rs_j Q_s Q_t^T with Q_s the S int8 digit planes
  * (each rows x K, row-major, host).  rows % 256 == 0, K % 128 == 0.  Used by the parity tests only. */
 int b200gp_i8_update_test(b200gp_ctx* ctx, const int8_t* planes, int S, int64_t rows, int64_t K,
@@ -194,7 +192,7 @@ int b200gp_dense_log_probability_batched(b200gp_ctx* ctx, const double* progs, i
  * panel(J); then finish().  Every rank ends up with the complete factor. */
 typedef struct b200gp_mg b200gp_mg;
 /* streaming != 0: keep no np x np fp64 matrix (rolling np x nb column buffer; the forward solve and log-det
- * are folded into each panel step) -- only the int8 digit planes stay resident (N = 131072 fits one B200). */
+ * are folded into each panel step) -- only the int8 digit planes stay resident (S N^2 bytes per GPU). */
 int b200gp_mg_create(b200gp_ctx* ctx, const double* prog, int n_instr, const double* X, int64_t n, int ndim,
                      const double* diag, const double* resid, int slices, int streaming, b200gp_mg** out);
 int b200gp_mg_free(b200gp_mg* m);

@@ -1,5 +1,5 @@
 """`jax.random` stand-in: NumPy generators behind key objects.  Streams differ from threefry by construction, so
-sample *values* are not reference values — only their statistics are (SURVEY §8 a19)."""
+sample *values* are not reference values — only their statistics are."""
 
 import numpy as _np
 

@@ -1,4 +1,4 @@
-"""Full-size LAPACK known answers for the bench workloads (SURVEY 8(d): "65 536 one-off golden").
+"""Full-size LAPACK known answers for the bench workloads (one-off, N = 65 536).
 
     python tests/golden/make_golden_full.py c2      # N=65536 ExpSquared, the bench default (about 30 min, 35 GB)
     python tests/golden/make_golden_full.py c3s     # N=65537 Matern52+RationalQuadratic (L2), the sharded workload

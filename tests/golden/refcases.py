@@ -1,6 +1,6 @@
 """Reference-generated golden cases: one definition, three executors.
 
-`run_case(ns, case)` drives a `GaussianProcess` API through the quantities of SURVEY §8(a).  The *same* kernel
+`run_case(ns, case)` drives a `GaussianProcess` API through the quantities it exposes.  The *same* kernel
 expression strings are evaluated against
 
   * the unmodified reference (`tinygp` from /root/reference over tests/golden/jaxshim) -> make_golden_reference.py

@@ -1,7 +1,7 @@
 """The plugin boundary, literally: the UNMODIFIED reference `tinygp.GaussianProcess` (from /root/reference, over the
 NumPy stand-ins for jax/equinox in tests/golden/jaxshim) driven with `solver=tinygp_b200.adapter.DirectSolver /
 QuasisepSolver`.  tinygp's own gp.py makes every call (constructor with `covariance=`, the six Solver methods, the
-Conditioned kernel calling back into `solve_triangular`); the B200 host layer answers, here over the mock C-ABI
+Conditioned kernel calling back into `solve_triangular`); the tinygp_b200 host layer answers, here over the mock C-ABI
 (tests/hostmock.py) because this container has no GPU and the GPU box has no reference checkout.  Results must equal
 what the reference computes with its own solvers."""
 

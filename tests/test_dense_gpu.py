@@ -1,4 +1,4 @@
-"""Parity of the CUDA DirectSolver path against the oracle (run with -m gpu on the B200 box).
+"""Parity of the CUDA DirectSolver path against the oracle (run with -m gpu on an H100).
 Everything goes through the C-ABI (ctypes) exactly as a user of the plugin surface would."""
 
 import numpy as np
@@ -219,9 +219,12 @@ def test_sampling_statistics():
 
 @pytest.mark.parametrize("slices", [8, 0])
 def test_large_n_properties(ctx, slices):
-    """N = 8192: parity against the oracle (LAPACK dpotrf, ~3 s) plus size-independent identities, for the
-    default int8 fixed-point trailing update (8 digit planes) and for the native fp64 DMMA path."""
+    """N = 8192: parity against the oracle (LAPACK dpotrf, ~3 s) plus size-independent identities, for the int8
+    fixed-point trailing update (8 digit planes, forced on with ozaki_min_n = 0) and for the native fp64 DMMA path
+    (the default)."""
     ctx.set_option("ozaki_slices", slices)
+    if slices:
+        ctx.set_option("ozaki_min_n", 0)
     rng = np.random.default_rng(49382)
     n = 8192
     X = rng.uniform(0, 10, (n, 3))

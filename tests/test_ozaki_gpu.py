@@ -1,5 +1,5 @@
-"""The int8 fixed-point (Ozaki-style) trailing update on tcgen05: exactness of the integer products, digit
-cutting, and parity of the full factorisation against the oracle (run with -m gpu on the B200 box)."""
+"""The int8 fixed-point (Ozaki-style) trailing update on the wgmma tensor cores: exactness of the integer products, digit
+cutting, and parity of the full factorisation against the oracle (run with -m gpu on an H100)."""
 
 import numpy as np
 import pytest
@@ -29,7 +29,7 @@ def test_i8_update_kernel_is_exact(ctx, rows, K, S, cluster, pairing, layout):
     2 = the paired loop structure with single groups (diagnostic).  layout: 0 = plane-major digit planes,
     1 = chunk-major (all planes of a 128-byte K chunk adjacent; one 4-D tensor map)."""
     if (pairing or layout) and cluster in (1, 2):
-        pytest.skip("the wide variant has neither switch; the paired CTA-pair kernel is tested in test_zz_*")
+        pytest.skip("the wide variant has neither switch; the paired default launch is tested in test_zzz_*")
     ctx.set_option("ozaki_cluster", cluster)
     ctx.set_option("ozaki_pairing", pairing)
     ctx.set_option("ozaki_layout", layout)
@@ -88,7 +88,7 @@ def test_ozaki_layout_and_pairing_variants(ctx, layout, pairing):
     k = 1.3 * kernels.ExpSquared(0.8)
     ctx.set_option("nb", 512)
     ctx.set_option("ozaki_min_n", 0)
-    ctx.set_option("ozaki_cluster", 21)       # the chunk-major layout exists for the cta_group::1 kernels only
+    ctx.set_option("ozaki_cluster", 21)
     ctx.set_option("ozaki_layout", layout)
     ctx.set_option("ozaki_pairing", pairing)
     try:

@@ -1,5 +1,5 @@
 """The N > 1 host logic (problem sharding, max-over-ranks timing, result gather) on CPU with gloo, world_size 2.
-The data path itself has no collective (replicas); see DESIGN.md section 5."""
+The data path itself has no collective (replicas)."""
 
 import os
 

@@ -1,4 +1,4 @@
-"""Parity of the CUDA QuasisepSolver path against the oracle (run with -m gpu on the B200 box)."""
+"""Parity of the CUDA QuasisepSolver path against the oracle (run with -m gpu on an H100)."""
 
 from ctypes import byref, c_int, c_void_p
 

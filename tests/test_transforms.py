@@ -1,4 +1,4 @@
-"""Input transforms (SURVEY row f3; reference: src/tinygp/transforms.py:23-161, docs in transforms.py:44-55,
+"""Input transforms (reference: src/tinygp/transforms.py:23-161, docs in transforms.py:44-55,
 81-92,143-154).  CPU tests check the host lowering (per-leaf metric matrices, augmented columns) through a
 Python restatement of the device interpreter; GPU tests check the CUDA build kernels and the full
 GaussianProcess path against the oracle, which maps the *points* like the reference does."""
@@ -202,7 +202,7 @@ def test_gp_with_transforms_gpu(name):
 
 @pytest.mark.gpu
 def test_transforms_int8_path_gpu():
-    """the tcgen05 fixed-point factorisation sees the same build kernel: force it at a small size"""
+    """the int8 fixed-point factorisation sees the same build kernel: force it at a small size"""
     import tinygp_b200 as tg
     from tinygp_b200 import _cabi
     _, k, kr, nd = next(c for c in CASES if c[0] == "cholesky_mat")

@@ -1,7 +1,5 @@
-"""GPU cases that execute device code (or launch logic) written or changed AFTER round 1's last GPU run -- everything else
-in the `-m gpu` suite runs machine code that is byte-identical to what already passed on the B200
-(profiles/r1_head_check.md).  This file sorts last so that a first-run surprise here cannot hide the other results under
-the driver's `pytest -x`:
+"""GPU cases for the newer device code paths.  This file sorts late so that a surprise here cannot hide the other results
+under `pytest -x`:
   * QuasisepSolver conditioning on the device (`b200gp_qs_condition`), diag((K + N)^-1) and the O(N) conditioned variance
     (GramBack backward scan; its source passes on the CPU in tests/test_device_code_on_host.py);
   * the K-range split of the int8 update, the panel-overlap / build-ahead options, the warp-shuffle tree option;

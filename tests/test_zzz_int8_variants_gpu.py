@@ -1,7 +1,7 @@
-"""int8 update kernel variants whose device code changed or was written after round 1's last GPU run: the paired-group
-kernels `i8_update_kernel<CM, CN, true>` (pairing order for odd plane counts changed) and the new paired CTA-pair kernel
-`i8_update_kernel_2sm<true>`.  Last file of the `-m gpu` suite on purpose: if a brand-new tcgen05 kernel faulted, the CUDA
-context of the test process would be unusable for whatever came after it."""
+"""int8 update kernel variants: the paired-group kernels `i8_update_kernel<CM, CN, true, 1>` for every cluster shape, the
+default 2 x 1 cluster launch (ozaki_cluster = 2) with and without pairing, and its split-K segments.  Last file of the
+`-m gpu` suite on purpose: if a kernel faulted, the CUDA context of the test process would be unusable for whatever came
+after it."""
 
 import numpy as np
 import pytest
@@ -18,9 +18,8 @@ pytestmark = pytest.mark.gpu
 @pytest.mark.parametrize("cluster", [11, 21, 12, 22, 41, 42])
 @pytest.mark.parametrize("rows,K,S", [(256, 128, 1), (256, 512, 3), (512, 1024, 8), (768, 384, 7), (512, 2048, 2)])
 def test_paired_group_kernels_are_exact(ctx, rows, K, S, cluster, pairing, layout):
-    """i8_update_kernel<CM, CN, true>: two digit groups per pass (pairing 1) and its single-group diagnostic (2).  These
-    passed on the B200 with the previous pairing order; the order for odd S changed after the last GPU run (the
-    unpaired group is now group 0), hence their place in this file."""
+    """i8_update_kernel<CM, CN, true, 1>: two digit groups per pass (pairing 1) and its single-group diagnostic (2); for an
+    odd plane count the unpaired group is group 0."""
     from test_ozaki_gpu import _ref_update
     from tinygp_b200 import _cabi
     ctx.set_option("ozaki_cluster", cluster)
@@ -50,7 +49,7 @@ def test_factorisation_with_paired_groups(ctx, layout, pairing):
     k = 1.3 * kernels.ExpSquared(0.8)
     ctx.set_option("nb", 512)
     ctx.set_option("ozaki_min_n", 0)
-    ctx.set_option("ozaki_cluster", 21)       # the chunk-major layout exists for the cta_group::1 kernels only
+    ctx.set_option("ozaki_cluster", 21)
     ctx.set_option("ozaki_layout", layout)
     ctx.set_option("ozaki_pairing", pairing)
     try:
@@ -61,13 +60,12 @@ def test_factorisation_with_paired_groups(ctx, layout, pairing):
     assert rel(lp, lpo) < LOGP_RTOL, (lp, lpo)
 
 
-# last on purpose: a brand-new tcgen05 kernel; if it faulted, the CUDA context of this process would be unusable
 @pytest.mark.parametrize("pairing", [1, 2])
 @pytest.mark.parametrize("rows,K,S", [(256, 128, 1), (256, 512, 3), (512, 1024, 8), (768, 384, 7), (512, 2048, 2),
                                       (1024, 4096, 7)])
 def test_paired_cta_pair_kernel_is_exact(ctx, rows, K, S, pairing):
-    """i8_update_kernel_2sm<true>: tcgen05 cta_group::2 with two digit groups per pass (written after round 1's last GPU
-    run; same exactness harness as tests/test_ozaki_gpu.py::test_i8_update_kernel_is_exact)"""
+    """the default launch shape (ozaki_cluster = 2: 2 x 1 cluster, B slices multicast) with two digit groups per pass (same
+    exactness harness as tests/test_ozaki_gpu.py::test_i8_update_kernel_is_exact)"""
     from tinygp_b200 import _cabi
     ctx.set_option("ozaki_cluster", 2)
     ctx.set_option("ozaki_pairing", pairing)
@@ -92,7 +90,7 @@ def test_paired_cta_pair_kernel_is_exact(ctx, rows, K, S, pairing):
 @pytest.mark.parametrize("force", [2, 3, 5])
 @pytest.mark.parametrize("rows,K,S", [(512, 1024, 7), (768, 1920, 7), (1024, 4096, 8), (256, 640, 3)])
 def test_split_k_segments_are_exact(ctx, rows, K, S, force):
-    """CTA-pair kernel with the K range cut into segments inside one launch (segment 0 updates C, the others their own
+    """default launch shape with the K range cut into segments inside one launch (segment 0 updates C, the others their own
     zero-filled scratch tiles, added afterwards in a fixed order): same integer sums, one more fp64 addition per segment"""
     from tinygp_b200 import _cabi
     ctx.set_option("ozaki_cluster", 2)

@@ -1,7 +1,7 @@
-"""tinygp_b200 -- a B200-native solver backend behind tinygp's plugin surface.
+"""tinygp_b200 -- an H100-native (sm_90a) solver backend behind tinygp's plugin surface.
 
 ``GaussianProcess`` / ``kernels`` / ``noise`` / ``solvers`` mirror ``tinygp``'s names
-(src/tinygp/__init__.py); the arithmetic runs in hand-written sm_100a CUDA behind the C-ABI of
+(src/tinygp/__init__.py); the arithmetic runs in hand-written sm_90a CUDA behind the C-ABI of
 ``include/b200gp.h``.  There is no CPU fallback.  ``adapter.DirectSolver`` / ``adapter.QuasisepSolver`` accept the
 reference's own kernel / noise objects and can be passed as ``solver=`` to ``tinygp.GaussianProcess``.
 """

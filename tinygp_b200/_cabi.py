@@ -50,7 +50,6 @@ SIGNATURES = {
     "b200gp_get_profile": (c_int, [c_void_p, POINTER(Profile), c_int]),
     "b200gp_measure_fp64_peak": (c_int, [c_void_p, c_double_p, c_double_p]),
     "b200gp_measure_i8_peak": (c_int, [c_void_p, c_double_p]),
-    "b200gp_measure_i8_peak_2sm": (c_int, [c_void_p, c_double_p]),
     "b200gp_i8_update_test": (c_int, [_V, _D, _I, _L, _L, _D, _D]),
     "b200gp_i8_update_bench": (c_int, [_V, _L, _L, _L, _I, _I, _L, _L, c_double_p, c_void_p]),
     "b200gp_kernel_matrix": (c_int, [_V, _D, _I, _D, _L, _D, _L, _I, _D]),

@@ -59,13 +59,13 @@ struct b200gp_ctx {
     b200gp_profile prof{};
     std::vector<CachedBuf> cache;  // freed big buffers kept for reuse
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    int num_sms = 148;
+    int num_sms = 132;
     int64_t peak_iters = 4096;  // loop length of the fp64 peak micro-benchmarks
     int64_t qs_chunk_max = 256; // upper end of the automatic chunk-length search of the quasiseparable scans
     int64_t qs_chunk = 0;       // points per thread in the quasiseparable scans (0 = chosen per problem size, see qs_create_impl)
     int64_t qsm_chunk = 0;      // points per warp in the QSM-algebra scans (qsm.cu); 0 = chosen per problem size
     int64_t qsm_sequential_redos = 0;   // read-only counter: Riccati scans redone sequentially after the consistency check (qsm.cu run_ric)
-    int64_t qs_tree = 1;        // 1: warp-shuffle scan over the chunk composites (fan-in 32; default: 0.95 vs 1.37 ms at N = 1e7), 0: thread-sequential fan-in-16 tree
+    int64_t qs_tree = 1;        // 1: warp-shuffle scan over the chunk composites (fan-in 32; default), 0: thread-sequential fan-in-16 tree
     int64_t potf2_version = 2;  // 1: column-at-a-time diagonal-block kernel, 2: rank-8 blocked with register tiles
     int64_t qs_kernel = 1;      // quasiseparable factorisation: 1 = layout-specialised kernels (qs_fast.cuh) when the model's block
                                 // layout is compiled in, 0 = always the generic J x J kernels of qs_core.cuh
@@ -73,17 +73,15 @@ struct b200gp_ctx {
     int64_t build_fast = 2;     // kernel-matrix build: 2 = + compile-time single-leaf kernels (coef * one stationary leaf, <= 3-D),
                                 // 1 = sum-of-products normal form when the program has one, 0 = interpreter
     int64_t panel_fused = 0;    // 1: one launch per 128-column step of the panel factorisation (potf2 + trtri + solve)
-    int64_t oz_splitk = 1024;   // int8 update (CTA-pair kernel): > 0 = split K over idle SM pairs, value = fixed cost of a tile in K
+    int64_t oz_splitk = 1024;   // int8 update (default launch shape): > 0 = split K over idle SM pairs, value = fixed cost of a tile in K
                                 // columns for the policy (ozaki.cu choose_splitk); 0 = one K range per tile
     int64_t mg_splitk = 0;       // sharded path: 0 (default) = one K range per tile: bit-identical results for every rank count;
-                                 // 1 = tail split-K on every rank's rows too (2 GPUs, N = 131072: update 2791 -> 2738 ms, step not faster)
-    int64_t oz_splitk_force = 0; // > 1: that many K segments in every CTA-pair launch (tests)
+                                 // 1 = tail split-K on every rank's rows too (the summation order then depends on the rank count)
+    int64_t oz_splitk_force = 0; // > 1: that many K segments in every default-shape launch (tests)
     int64_t nb_batched = 4096;  // outer panel width of the batched small-N driver: 4096 = N of config 5, i.e. one left-looking sweep (reads C
-                                // once per 128-column block); measured 843 / 956 / 1025 / 1055 / 1061 logp/s for 256 / 512 / 1024 / 2048 / 4096
-    // > 0: int8 fixed-point trailing update with this many digit planes (ozaki.cu); 0 = DMMA.  7 planes = 48 bits under the
-    // row scale: at N = 65536 the log-probability differs from the LAPACK golden by 4.7e-12 with 7 AND with 8 planes
-    // (profiles/r1_bench_dense_int8x{7,8}.json vs tests/golden/full_size.json) -- the digit truncation is below the fp64
-    // rounding of the factorisation itself, so the 8th plane buys nothing; 8 stays available (ozaki_slices).
+                                // once per 128-column block)
+    // > 0: int8 fixed-point trailing update with this many digit planes (ozaki.cu) once N >= oz_min_n; 0 = DMMA.  7 planes =
+    // 48 bits under the row scale, 8 = 55 bits (ozaki_slices).
     int64_t oz_slices = 7;
     int64_t oz_lookahead = 0;   // overlap the fp64 panel factorisation with the int8 update on a second stream
     cudaStream_t stream2 = nullptr;
@@ -99,19 +97,25 @@ struct b200gp_ctx {
     double* fuse_x = nullptr;             // np: L^-1 resid once the factorisation has returned
     int64_t solve_overlap = 1;            // option: 1 = hide the forward substitution of log_probability under the factorisation
     cudaStream_t stream_solve = nullptr;
-    int64_t panel_chain = 1;    // look-ahead panel: 1 (default) = right-looking order inside the diagonal block (chain 1.8 -> 1.3 ms per
-                                // panel: panel phase 166 -> 152 ms at N = 65536), 0 = left-looking (bit-identical to panel_overlap 0 / 1)
+    int64_t panel_chain = 1;    // look-ahead panel: 1 (default) = right-looking order inside the diagonal block (a shorter chain of
+                                // small kernels per panel), 0 = left-looking (bit-identical to panel_overlap 0 / 1)
     cudaStream_t stream_hi = nullptr;   // high-priority stream of the look-ahead panel chain (panel_overlap = 2)
     int64_t oz_prefetch = 0;    // L2 prefetch distance (K-chunks of 128) of the int8 update's TMA producer
     int64_t oz_pairing = 1;    // int8 update: 1 = accumulate two digit groups at once (default: 16 instead of 28 operand-stage loads
                                // per K chunk at 7 planes), 0 = one group per pass, 2 = diagnostic (paired loop order, single groups)
     int64_t oz_layout = 0;     // digit planes: 0 plane-major, 1 chunk-major (all planes of a K chunk adjacent)
-    int64_t oz_cluster = 2;     // int8 update kernel: 2 = CTA pair with tcgen05 cta_group::2 (default: 256 x 256 tile per pair, B halves
-                                // shared through the peer's shared memory), 1 = wide 1-SM tile, CM*10 + CN = cta_group::1 cluster shapes
+    int64_t oz_cluster = 2;     // int8 update kernel: 2 = 2 x 1 cluster with tail split-K (default: B slices multicast to the CTA below),
+                                // 1 = wide 256-row CTA tile, CM*10 + CN = cluster shapes of 128 x 128 CTA tiles (ozaki.cu)
     int64_t oz_subpanel = 0;    // two-level blocking of the int8 factorisation: fp64 panel width inside a block column (0 = off:
-                                // default; 256 / 512 measured within 0.5 % of look-ahead alone, see DESIGN.md section 3a)
+                                // default)
     int64_t oz_l2promo = 3;     // TMA L2 promotion of the digit-plane maps: 0 none, 1 64 B, 2 128 B, 3 256 B
-    int64_t oz_min_n = 8192;    // below this size the native DMMA path is used
+    // from this size on the int8 fixed-point update is used (with oz_slices > 0); below it the native DMMA path.  Default:
+    // never -- on an H100 (400 W) the DMMA factorisation is the faster one at N = 65536 (4.45 against 5.84 s per
+    // log_probability, 7 planes) and 40x closer to the LAPACK value; ozaki_min_n = 0 forces the int8 path.  The comparison
+    // is against an untuned int8 kernel (ozaki.cu): at 9 warps per CTA ptxas caps it at 168 registers, so the paired and
+    // wide variants spill, and each consumer warpgroup waits for its MMAs after every stage instead of keeping one wgmma
+    // group in flight; it reached 23 % of the resident-operand wgmma rate.
+    int64_t oz_min_n = (int64_t)1 << 40;
     // deferred (non-blocking) kernel timers: event pairs resolved at the next flush_timers()
     struct Pending { cudaEvent_t a, b; double* acc; };
     std::vector<Pending> pending;

@@ -1,4 +1,4 @@
-// Dense DirectSolver path for sm_100a: pairwise kernel build (K1), blocked right-looking Cholesky
+// Dense DirectSolver path for sm_90a: pairwise kernel build (K1), blocked right-looking Cholesky
 // whose panel/trailing updates run on the fp64 tensor pipe (DMMA, mma.sync.m8n8k4.f64) (K2),
 // triangular solves + reductions behind log_probability (K3), L@z (K4).
 //
@@ -48,8 +48,7 @@ struct BuildArgs {
 #define BUILD_ROWS 32
 #define BUILD_COLS 128
 // FAST: the program in sum-of-products normal form (kprog.cuh KFast) -- no interpreter loop, no stack in local memory.
-// ncu (round 2, N = 16384, 1.0 * ExpSquared): the interpreted version executes ~270 instructions per element with its
-// 8-entry value stack in local memory (2 x 2.0e8 local sectors) and reaches 11 % of the HBM write peak.
+// The interpreted version keeps its 8-entry value stack in local memory.
 template <bool FAST>
 __global__ void __launch_bounds__(256, 3) build_rect_kernel_t(const __grid_constant__ KProg P0, const __grid_constant__ KFast F0,
                                                              const BuildArgs a) {
@@ -113,9 +112,8 @@ __global__ void __launch_bounds__(256, 3) build_rect_kernel_t(const __grid_const
 }
 
 // SINGLE: coef * one stationary leaf, identity metric, 1-3 dimensions, everything about the program a template parameter --
-// the shape of BASELINE configs 1, 2, 5 (`amp * ExpSquared(scale)`) and of most hyper-parameter searches.  ncu of the
-// normal-form kernel above (profiles/r2_ncu_build.md): ~230 instructions per element, issue-bound at 12 % of the HBM write
-// peak, most of them loop / predicate / runtime-dispatch overhead around one fp64 exp.  Here a thread keeps its two columns'
+// the shape of the benchmark workloads (`amp * ExpSquared(scale)`) and of most hyper-parameter searches.  The normal-form
+// kernel above spends most of its instructions on loop / predicate / runtime-dispatch overhead around one fp64 exp.  Here a thread keeps its two columns'
 // coordinates in registers, the row coordinates come from shared memory as broadcasts, model constants are folded on the
 // host (1 / scale^2: one rounding in the argument, within the 1e-13 parity tolerance), and tiles that touch neither the
 // diagonal nor the padding run without a single predicate.  Boundary / diagonal tiles take the general element path.
@@ -611,7 +609,7 @@ __global__ void __launch_bounds__(PF_THREADS, 1) potf2_trtri_kernel(double* A, i
 }
 
 // ---- v2: rank-8 blocked right-looking Cholesky + 8-column blocked inverse, register tiles -------------------
-// v1 does 2 shared-memory loads per FMA (no register reuse) and 2-3 barriers per column: 186 us per block (ncu).
+// v1 does 2 shared-memory loads per FMA (no register reuse) and 2-3 barriers per column.
 // Here every 8-column panel is factored redundantly in registers by the threads that own its rows (no barrier
 // inside), the rank-8 trailing update uses 4x4 register tiles (2 FMA per load) and the inverse is built 8 columns
 // at a time: 32 + 48 barriers instead of 640.
@@ -656,7 +654,7 @@ __global__ void __launch_bounds__(PF_THREADS, 1) potf2_trtri_kernel_v2(double* A
             const int r = tid;
             int firstbad = -1;
             double invd[8];     // 1 / L_cc: the column is scaled by the reciprocal (as LAPACK's dpotf2 does with DSCAL), which
-                                // takes the 36 fp64 divisions per 8 x 8 block out of the serial chain (ncu: 158 us per call)
+                                // takes the 36 fp64 divisions per 8 x 8 block out of the serial chain
 #pragma unroll
             for (int c = 0; c < 8; ++c) {
                 double v = D[c][c];
@@ -901,7 +899,7 @@ void dense_panel_factor(b200gp_dense* s, int64_t k0, int64_t kb) {
 }
 
 // Look-ahead form of the panel factorisation (option "panel_overlap" = 2): the kb x kb DIAGONAL BLOCK is factored on the
-// main stream -- a chain of small kernels whose length is set by the serial 128 x 128 potf2 steps (~158 us each by ncu) --
+// main stream -- a chain of small kernels whose length is set by the serial 128 x 128 potf2 steps --
 // while the rows BELOW the block are updated / solved on a side stream, column by column, as soon as the potf2 of that
 // column has produced inv(L_jj).  The wide GEMMs no longer wait for the next potf2 and vice versa; per panel the time
 // becomes ~max(potf2 chain, wide GEMMs) instead of their sum.  Same tiles, same arithmetic: bit-identical results.
@@ -916,7 +914,7 @@ static void dense_panel_factor_lookahead(b200gp_dense* s, int64_t k0, int64_t kb
     cudaStream_t wide = ctx->stream;            // the caller's stream keeps the wide GEMMs (and the ProfTimer events)
     // The chain of small kernels runs on a HIGH-PRIORITY stream: when an SM frees up, the block scheduler then places the
     // chain's CTA before the pending CTAs of the wide GEMM grid.  (First attempt, chain on the default-priority stream and
-    // GEMMs on a side stream: no overlap at all -- the potf2 CTA queued behind every pending GEMM CTA: panel 212 vs 218 ms.)
+    // GEMMs on a side stream: no overlap at all -- the potf2 CTA queued behind every pending GEMM CTA.)
     if (!ctx->stream_hi) {
         int lo = 0, hi = 0;
         CUDA_CHECK(cudaDeviceGetStreamPriorityRange(&lo, &hi));
@@ -930,7 +928,7 @@ static void dense_panel_factor_lookahead(b200gp_dense* s, int64_t k0, int64_t kb
     // chain_right (option "panel_chain" = 1): RIGHT-looking order inside the diagonal block -- after the block column is
     // solved, the remaining (blk - 1) x (blk - 1) lower tiles of the block are updated with K = 128 (up to 28 tiles in
     // parallel) instead of updating each block column just before its potf2 with K = j0 (1-7 tiles, a single CTA running
-    // K = 896 takes 164 us).  Shorter chain per panel (1.8 -> ~1.3 ms by the launch list), different summation order of the
+    // the longest K).  Shorter chain per panel, different summation order of the
     // diagonal block (not bit-identical to the left-looking orders).
     const bool chain_right = (ctx->panel_chain == 1);
     for (int64_t j0 = 0; j0 < kb; j0 += TILE) {
@@ -1716,10 +1714,10 @@ static double dense_logp_impl(b200gp_ctx* ctx, const KProg& P, const double* X, 
     {
         // no factor is retained by this entry point, so very large problems stream their block columns (no N x N
         // fp64 matrix: only the digit planes stay resident).  Smaller ones keep the matrix: the rolling column
-        // buffer competes with the operand planes for L2 and costs ~10 % (measured at N = 65536).
+        // buffer competes with the operand planes for L2.
         const int64_t npad = ((n + TILE - 1) / TILE) * TILE;
         const double need = (double)npad * (double)npad * (8.0 + (double)ctx->oz_slices);
-        if (ctx->oz_slices > 0 && npad >= ctx->oz_min_n && need > 150e9)
+        if (ctx->oz_slices > 0 && npad >= ctx->oz_min_n && need > 70e9)     // 80 GB of HBM3
             return ozaki_logp_streaming(ctx, P, X, n, ndim, diag, resid, (int)ctx->oz_slices);
     }
     // the int8 factorisation runs the forward substitution itself, panel by panel on a side stream under the update of

@@ -1,26 +1,27 @@
-// Fixed-point (Ozaki-style) Cholesky update on the 5th-gen tensor cores: tcgen05.mma kind::i8, TMA-fed
-// operands, int32 accumulators in TMEM.
+// Fixed-point (Ozaki-style) Cholesky update on the Hopper tensor cores: wgmma s8 x s8 -> s32 with both operands in
+// shared memory, fed by TMA (multicast inside a thread-block cluster) through an mbarrier ring; int32 accumulators live
+// in registers.
 //
-// tcgen05 has no f64 kind, and the DMMA pipe sustains only ~30 TFLOP/s, so the N^3/3 flop of
-// `linalg.cholesky` (src/tinygp/solvers/direct.py:53) are moved onto the int8 tensor pipe:
+// The N^3/3 flop of `linalg.cholesky` (src/tinygp/solvers/direct.py:53) can be moved from the fp64 tensor pipe (DMMA)
+// onto the int8 tensor pipe:
 //
 //   * |L_ik| <= sqrt(K_ii) for a Cholesky factor, so every row of L has the a-priori scale
 //     rs_i = 2^ceil(log2 sqrt(K_ii)) and  x_ik = L_ik / rs_i  lies in [-1, 1].
 //   * x is cut into S signed 7-bit digits (first digit 6 bits):  x = sum_s q_s 2^-(6+7s) , q_s in int8,
 //     with exact remainders (every step is exact in fp64).  Digits are stored as S int8 planes.
 //   * sum_k L_ik L_jk = rs_i rs_j sum_{s,t} 2^-(12+7(s+t)) (q_s[i,:] . q_t[j,:])  where each integer dot
-//     product is EXACT in int32; pairs with equal s+t = g share one TMEM accumulator, pairs with
+//     product is EXACT in int32; pairs with equal s+t = g share one accumulator, pairs with
 //     s+t >= S are dropped (<= 2^-(6+7(S-1)) relative to the row scale: 2^-55 for S = 8).
 //   * left-looking block columns: column block J is generated (K tiles), then
 //     C -= L[rows, 0:c0] L[c0:c0+nb, 0:c0]^T runs with K = c0 (all previous panels at once), so each C tile
 //     is converted int32 -> fp64 only S times in total; then the panel is factored in fp64 on the DMMA
 //     path (dense.cu) and its digits are cut.
 //
-// Kernel (one CTA per 128 x 256 tile of C, 192 threads):
-//   warp 0   : TMA producer  (cp.async.bulk.tensor.2d, 128-byte swizzle, 4-stage mbarrier ring)
-//   warp 1   : TMEM alloc + single-thread tcgen05.mma issuer (M=128, N=256, K=32 per instruction)
-//   warps 2-5: epilogue: tcgen05.ld 32x32b -> cvt -> C -= rs_i rs_j 2^-(12+7g) G_g  (fp64 RMW on the tile)
-// Two 256-column accumulators ping-pong so the epilogue of group g overlaps the MMAs of group g+1.
+// Kernel (one CTA per 128 x 128 tile of C, or 256 x 128 for the wide variant; 288 threads):
+//   warps 0-3, 4-7: two consumer warpgroups; warpgroup c owns the rows [c * 64 MW, (c + 1) * 64 MW) of the tile and issues
+//                   wgmma.m64n128k32 from the ring stages, then converts its accumulators and updates C in fp64
+//   warp 8        : TMA producer (cp.async.bulk.tensor, 128-byte swizzle, 192 KB ring)
+// The two warpgroups work on the same stages independently, so the epilogue of one overlaps the MMAs of the other.
 #include "common.cuh"
 #include "kprog.cuh"
 #include <cuda.h>
@@ -28,25 +29,31 @@
 
 namespace oz {
 
-constexpr int TM = 128;          // tile rows  (UMMA M)
-constexpr int TN = 256;          // tile cols  (UMMA N)
+constexpr int TM = 128;          // rows of a launch tile (Args.tiles_m counts these)
+constexpr int TN = 256;          // columns of a launch tile (Args.tiles_n counts these)
+constexpr int CTN = 128;         // columns of one CTA tile (the wgmma N)
 constexpr int KC = 128;          // int8 K elements per pipeline stage (= one 128-byte swizzle row)
-constexpr int STAGES = 4;
-constexpr int A_BYTES = TM * KC;             // 16 KiB
-constexpr int B_BYTES = TN * KC;             // 32 KiB
-constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-constexpr int THREADS = 192;
+constexpr int B_BYTES = CTN * KC;            // 16 KiB
+constexpr int RING_BYTES = 192 * 1024;
+constexpr int THREADS = 288;                 // 2 consumer warpgroups + 1 producer warp
+constexpr int BOXR = 32;                     // rows per TMA box (a 4 x 1 cluster multicasts 32-row slices of B)
 constexpr uint32_t SPIN_LIMIT = 1u << 26;    // bounded waits: a protocol bug must not hang the GPU
 
-// instruction descriptor (cute/arch/mma_sm100_desc.hpp InstrDescriptor): c=S32, a=b=INT8, K-major, N=256, M=128
-constexpr uint32_t IDESC = (2u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(TN >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
+// MW = m64 blocks per consumer warpgroup: 1 (128-row CTA tile) or 2 (the wide 256-row tile)
+template <int MW>
+struct Geo {
+    static constexpr int ROWS = 128 * MW;
+    static constexpr int A_BYTES = ROWS * KC;
+    static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+    static constexpr int STAGES = RING_BYTES / STAGE_BYTES;              // 6 or 4
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+};
 
 struct Args {
     double* C; int64_t ldc;            // fp64 tile base: C[(row0 + i) * ldc + col0 + j]
     const double* rs;                  // row scales (power of two), indexed by global row
     int64_t row0, col0;                // global row / col of tile (0,0)
-    int tiles_m, tiles_n;
+    int tiles_m, tiles_n;              // TM x TN launch tiles
     int K;                             // int8 K extent (multiple of KC)
     int k_begin;                       // first K column (multiple of KC)
     int S;                             // number of digit planes used
@@ -58,23 +65,23 @@ struct Args {
     int pg_single;                     // diagnostic: paired-group loop structure (kc outer) with ONE group per pass
     int* error_flag;
     unsigned long long* dbg;           // optional in-kernel cycle counters (see DBG_* below); nullptr = off
-    // split-K of the tail tiles (CTA-pair kernel only; nseg <= 1 = off): pair indices >= split_from (ntail of them) are cut
-    // into nseg K segments of kseg columns that run as extra tiles of the SAME launch; segment 0 updates C, segment sg >= 1
-    // accumulates into its own zero-filled fp64 scratch tile Cseg[(sg - 1) * ntail + tail index][256][256] that
-    // splitk_fixup_kernel adds to C afterwards in a fixed order.
+    // split-K of the tail cluster tiles (nseg <= 1 = off): cluster indices >= split_from (ntail of them) are cut into nseg K
+    // segments of kseg columns that run as extra clusters of the SAME launch; segment 0 updates C, segment sg >= 1
+    // accumulates into its own zero-filled fp64 scratch tile Cseg[(sg - 1) * ntail + tail index][rows][cols] of the cluster
+    // tile that splitk_fixup_kernel adds to C afterwards in a fixed order.
     int nseg, kseg, split_from, ntail;
     double* Cseg;
     int no_split;                      // launcher hint: keep one K range per tile (sharded path: bit-identical for any rank count)
 };
 
-// in-kernel cycle counters (diagnostics, option-free: on when Args.dbg != nullptr).  Sums over CTAs of clock64() deltas.
+// in-kernel cycle counters (diagnostics, option-free: on when Args.dbg != nullptr).  Sums over CTAs of clock64() deltas;
+// the MMA / EPI slots are taken by consumer warpgroup 0.
 enum { DBG_PROD_WAIT = 0, DBG_PROD_TOTAL = 1, DBG_MMA_WAIT_FULL = 2, DBG_MMA_WAIT_TEMPTY = 3, DBG_MMA_TOTAL = 4,
        DBG_EPI_WAIT_TFULL = 5, DBG_EPI_TOTAL = 6, DBG_CTAS = 7, DBG_CTA_TOTAL = 8, DBG_N = 16 };
 
-// `all`: ONE 3-D map (k, row, plane) used by the main kernel -- cycling through per-plane descriptors makes every
-// TMA issue miss the descriptor cache (measured: 3x the per-stage cost once stages alternate planes);
-// `plane[s]`: 2-D per-plane maps kept for the wide / 2-SM variants.
-struct Maps { CUtensorMap all; CUtensorMap plane[8]; };
+// ONE 3-D map (k, row, plane) -- or 4-D for the chunk-major layout -- serves every stage: cycling through per-plane
+// descriptors would make every TMA issue miss the descriptor cache
+struct Maps { CUtensorMap all; };
 
 // ---- PTX wrappers -----------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -86,6 +93,14 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
 }
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ uint32_t mapa(uint32_t local_addr, uint32_t rank) {
+    uint32_t r;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;\n" : "=r"(r) : "r"(local_addr), "r"(rank));
+    return r;
+}
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
+    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];\n" ::"r"(cluster_addr) : "memory");
 }
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
     uint32_t ok;
@@ -119,13 +134,6 @@ __device__ __forceinline__ bool mbar_wait_t(uint64_t* bar, uint32_t parity, vola
 __device__ __forceinline__ void dbg_add(unsigned long long* dbg, int slot, unsigned long long v) {
     if (dbg) atomicAdd(dbg + slot, v);
 }
-__device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];\n" ::"r"(
-            smem_u32(smem_dst)),
-        "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-        : "memory");
-}
 __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2) {
     asm volatile(
         "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];\n" ::"r"(
@@ -136,61 +144,6 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
 __device__ __forceinline__ void tma_prefetch_3d(const CUtensorMap* map, int c0, int c1, int c2) {
     asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];\n" ::"l"(map), "r"(c0), "r"(c1), "r"(c2)
                  : "memory");
-}
-// fire-and-forget L2 prefetch of a TMA box: the demand loads of the shared-memory ring then see L2-hit latency
-// instead of loaded DRAM latency (the ring holds only 192 KB; ncu showed the kernel latency-bound)
-__device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap* map, int c0, int c1) {
-    asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];\n" ::"l"(map), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void umma_i8(uint32_t tmem_c, uint64_t da, uint64_t db, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_c),
-        "l"(da), "l"(db), "r"(IDESC), "r"(accumulate)
-        : "memory");
-}
-// K-major operand, 128-byte swizzle: SBO = 1024 B between 8-row groups, LBO unused (=1), version 1 (sm100)
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)1 << 16;                 // leading byte offset (ignored for swizzled K-major)
-    d |= (uint64_t)(1024 >> 4) << 32;       // stride byte offset
-    d |= (uint64_t)1 << 46;                 // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;                 // SWIZZLE_128B
-    return d;
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-}
-
-// ---- the tile kernel ----------------------------------------------------------------------------
-// Cluster of CM x CN CTAs (cluster rank r: cm = r % CM, cn = r / CM) working on CM x CN neighbouring tiles.
-// The A tile (rows of ti) is needed by the CN CTAs of a cluster row and the B tile (rows of tj) by the CM
-// CTAs of a cluster column: every CTA fetches only its 1/CN slice of A and 1/CM slice of B and TMA-multicasts
-// it to its mates, which divides the L2 -> SM traffic (the measured bottleneck of the 1 x 1 version).
-__device__ __forceinline__ void tma_load_2d_mc(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1,
-                                               uint16_t mask) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-        " [%0], [%1, {%3, %4}], [%2], %5;\n" ::"r"(smem_u32(smem_dst)),
-        "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask)
-        : "memory");
 }
 __device__ __forceinline__ void tma_load_3d_mc(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2,
                                                uint16_t mask) {
@@ -215,67 +168,110 @@ __device__ __forceinline__ void tma_load_4d_mc(void* smem_dst, const CUtensorMap
         "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "h"(mask)
         : "memory");
 }
-__device__ __forceinline__ void tc_commit_mc(uint64_t* bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n" ::"r"(
-                     smem_u32(bar)),
-                 "h"(mask)
-                 : "memory");
-}
 __device__ __forceinline__ void cluster_sync_all() {
     asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
     asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
 }
 
-constexpr int BOXR = 64;  // rows per TMA box
+// K-major operand, 128-byte swizzle (the layout TMA writes with CU_TENSOR_MAP_SWIZZLE_128B): stride byte offset 1024 B
+// between 8-row groups, leading byte offset unused; stage bases are 1024-byte aligned, so the base offset is 0 and a K step
+// of 32 bytes inside the swizzle atom is a plain advance of the start address
+__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
+    uint64_t d = 0;
+    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
+    d |= (uint64_t)1 << 16;
+    d |= (uint64_t)(1024 >> 4) << 32;
+    d |= (uint64_t)1 << 62;                 // SWIZZLE_128B
+    return d;
+}
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;\n" ::: "memory"); }
+__device__ __forceinline__ void wg_wait1() { asm volatile("wgmma.wait_group.sync.aligned 1;\n" ::: "memory"); }
 
-// ---- epilogue of one digit group (or a pair of groups) for this thread's tile row ----------------------------------
-// C[row, col0 + 0..255] += sc * rs_j * (acc0 + 2^-7 acc1).  The read-modify-write is issued in BATCHES: all loads of a
-// batch first, then the arithmetic, then the stores.  Round 1 had "load, fma, store" per 16 bytes with the row scales read
-// through a plain pointer, so every store could alias the next load and the accesses were serialised at the loaded
-// L2 latency (in-kernel counters, round 2: ~1.4 M cycles per 128 x 256 tile pass, i.e. ~9000 cycles per 16-byte RMW).
+// d (64 x 128 int32, 64 registers per thread) (+)= A (64 x 32 int8) B (128 x 32 int8)^T
+__device__ __forceinline__ void wgmma_i8(uint32_t (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p;\n\t}\n"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+          "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+          "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+          "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),
+          "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),
+          "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
+          "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
+          "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+        : "l"(da), "l"(db), "r"(accumulate)
+        : "memory");
+}
+
+// one stage (K = 128) of one m64 block: four k32 instructions
+__device__ __forceinline__ void mma_stage(uint32_t (&d)[64], uint32_t a_addr, uint32_t b_addr, uint32_t& accumulate) {
+#pragma unroll
+    for (int kk = 0; kk < KC / 32; ++kk) {
+        wgmma_i8(d, make_desc(a_addr + kk * 32), make_desc(b_addr + kk * 32), accumulate);
+        accumulate = 1;
+    }
+}
+
+// ---- epilogue of one digit group (or a pair of groups) for one m64 block ------------------------------------------
+// Accumulator fragment of wgmma m64nN (32-bit): thread (warp w, lane l) holds rows 16 w + l / 4 (registers 4 i, 4 i + 1)
+// and 16 w + l / 4 + 8 (4 i + 2, 4 i + 3) at columns 8 i + 2 (l % 4) + {0, 1}.
+// C[row, col] += sc_row * rs_col * (acc0 + 2^-7 acc1).  The read-modify-write is issued in batches (loads first, then the
+// arithmetic, then the stores), so that consecutive 16-byte accesses are not serialised on a possible alias.
 template <bool TWO>
-__device__ __forceinline__ void epi_rmw_row(uint32_t taddr0, uint32_t taddr1, double* __restrict__ crow,
-                                            const double* __restrict__ rs, int64_t gcol0, int64_t n_cols, bool row_ok,
-                                            double sc) {
-#pragma unroll 1
-    for (int cb = 0; cb < TN / 32; ++cb) {
-        uint32_t r0[32], r1[32];
-        tmem_ld32(taddr0 + (uint32_t)(cb * 32), r0);
-        if (TWO) tmem_ld32(taddr1 + (uint32_t)(cb * 32), r1);
-        const int64_t gc = gcol0 + cb * 32;
-        if (row_ok && gc < n_cols) {
+__device__ __forceinline__ void epi_rmw(const uint32_t (&d0)[64], const uint32_t (&d1)[64], double* crow0, double* crow1,
+                                        const double* __restrict__ rs, int64_t gc_lane, int64_t n_cols, bool ok0, bool ok1,
+                                        double sc0, double sc1) {
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {       // two batches of 16 columns: 8 + 8 independent 16-byte loads in flight
-                double2 cv[8], rj[8];
+    for (int ib = 0; ib < CTN / 8; ib += 4) {
+        double2 c0v[4], c1v[4], rj[4];
 #pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    cv[j] = *reinterpret_cast<const double2*>(crow + gc + h * 16 + 2 * j);
-                    rj[j] = __ldg(reinterpret_cast<const double2*>(rs + gc + h * 16 + 2 * j));
-                }
+        for (int j = 0; j < 4; ++j) {
+            const int64_t gc = gc_lane + 8 * (ib + j);
+            const bool in = gc < n_cols;
+            rj[j] = in ? __ldg(reinterpret_cast<const double2*>(rs + gc)) : make_double2(0.0, 0.0);
+            c0v[j] = (in && ok0) ? *reinterpret_cast<const double2*>(crow0 + gc) : make_double2(0.0, 0.0);
+            c1v[j] = (in && ok1) ? *reinterpret_cast<const double2*>(crow1 + gc) : make_double2(0.0, 0.0);
+        }
 #pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const int e = h * 16 + 2 * j;
-                    double tx = (double)(int)r0[e], ty = (double)(int)r0[e + 1];
-                    if (TWO) {   // group g0 + 1 is 2^-7 of group g0: a0 + a1 2^-7 is exact (|a| < 2^31), one rounding per pair
-                        tx = fma((double)(int)r1[e], 0.0078125, tx);
-                        ty = fma((double)(int)r1[e + 1], 0.0078125, ty);
-                    }
-                    cv[j].x = fma(sc * rj[j].x, tx, cv[j].x);
-                    cv[j].y = fma(sc * rj[j].y, ty, cv[j].y);
-                }
+        for (int j = 0; j < 4; ++j) {
+            const int e = 4 * (ib + j);
+            double t0x = (double)(int)d0[e], t0y = (double)(int)d0[e + 1];
+            double t1x = (double)(int)d0[e + 2], t1y = (double)(int)d0[e + 3];
+            if (TWO) {   // group g0 + 1 is 2^-7 of group g0: a0 + a1 2^-7 is exact (|a| < 2^31), one rounding per pair
+                t0x = fma((double)(int)d1[e], 0.0078125, t0x);
+                t0y = fma((double)(int)d1[e + 1], 0.0078125, t0y);
+                t1x = fma((double)(int)d1[e + 2], 0.0078125, t1x);
+                t1y = fma((double)(int)d1[e + 3], 0.0078125, t1y);
+            }
+            c0v[j].x = fma(sc0 * rj[j].x, t0x, c0v[j].x);
+            c0v[j].y = fma(sc0 * rj[j].y, t0y, c0v[j].y);
+            c1v[j].x = fma(sc1 * rj[j].x, t1x, c1v[j].x);
+            c1v[j].y = fma(sc1 * rj[j].y, t1y, c1v[j].y);
+        }
 #pragma unroll
-                for (int j = 0; j < 8; ++j) *reinterpret_cast<double2*>(crow + gc + h * 16 + 2 * j) = cv[j];
+        for (int j = 0; j < 4; ++j) {
+            const int64_t gc = gc_lane + 8 * (ib + j);
+            if (gc < n_cols) {
+                if (ok0) *reinterpret_cast<double2*>(crow0 + gc) = c0v[j];
+                if (ok1) *reinterpret_cast<double2*>(crow1 + gc) = c1v[j];
             }
         }
     }
 }
 
-
-// PG ("paired groups"): two digit groups g0 = 2P, g1 = 2P + 1 are accumulated at once in the two TMEM accumulators.
+// PG ("paired groups"): two digit groups g0 = 2P, g1 = 2P + 1 are accumulated at once in two register accumulators.
 // Per K chunk the ring then carries stages i = 0..g1 holding (A plane i, B plane g1 - i); stage i feeds
 //   A_i x B_{g1-i} -> accumulator 1 (group g1)   and   A_{i-1} (previous stage) x B_{g1-i} -> accumulator 0 (group g0),
-// so S = 8 needs 20 stage loads per K chunk instead of 36: the L2 -> shared-memory operand stream, which bounds the
-// unpaired kernel at ~50 % tensor-pipe utilisation (profiles/r1_ncu_i8_update.md), shrinks 1.8x for the same MMAs.
+// so S = 8 needs 20 stage loads per K chunk instead of 36 for the same MMAs.
 // Pass P of the paired loop covers digit group g0 and, if `two`, g0 + 1.  A paired pass streams g1 + 1 stages per K chunk
 // and a single pass g0 + 1, so for an odd plane count the UNPAIRED group is the cheap group 0, not the expensive last one:
 // S = 7 -> (0) (1,2) (3,4) (5,6) = 1 + 3 + 5 + 7 = 16 stage loads per K chunk for the 28 pair products (instead of
@@ -288,42 +284,53 @@ __device__ __forceinline__ void pg_pass(int S, int pg_single, int P, int& g0, bo
     two = (g0 + 1 < S);
 }
 
-template <int CM, int CN, bool PG>
+// ---- the tile kernel ----------------------------------------------------------------------------
+// Cluster of CM x CN CTAs (cluster rank r: cm = r % CM, cn = r / CM) working on CM x CN neighbouring CTA tiles.
+// The A tile (rows of ti) is needed by the CN CTAs of a cluster row and the B tile (rows of tj) by the CM
+// CTAs of a cluster column: every CTA fetches only its 1/CN slice of A and 1/CM slice of B and TMA-multicasts
+// it to its mates, which divides the L2 -> SM operand traffic.
+// A stage slot of CTA X is written by X's row and column mates, so X's consumers release it on the `empty` barrier of
+// each of them (2 warpgroups x (CM + CN - 1) arrivals per phase).
+template <int CM, int CN, bool PG, int MW>
 __global__ void __launch_bounds__(THREADS, 1) i8_update_kernel(const __grid_constant__ Maps maps, const Args g) {
-    static_assert((TM / CN) % BOXR == 0 && (TN / CM) % BOXR == 0, "slice must be whole TMA boxes");
+    using G = Geo<MW>;
+    constexpr int ROWS = G::ROWS, A_BYTES = G::A_BYTES, STAGE_BYTES = G::STAGE_BYTES, STAGES = G::STAGES;
+    static_assert((ROWS / CN) % BOXR == 0 && (CTN / CM) % BOXR == 0, "slice must be whole TMA boxes");
+    static_assert(!(PG && MW > 1), "two accumulators of two m64 blocks do not fit the register file");
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
     uint64_t* full = bars;                  // [STAGES]
     uint64_t* empty = bars + STAGES;        // [STAGES]
-    uint64_t* tfull = bars + 2 * STAGES;    // [2]
-    uint64_t* tempty = bars + 2 * STAGES + 2;  // [2]
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
-    volatile int* abort_flag = reinterpret_cast<volatile int*>(tmem_ptr + 1);
+    volatile int* abort_flag = reinterpret_cast<volatile int*>(bars + 2 * STAGES);
 
     constexpr int CS = CM * CN;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     int crank = 0;
     if (CS > 1) asm volatile("mov.u32 %0, %%cluster_ctarank;\n" : "=r"(crank));
     const int cm = crank % CM, cn = crank / CM;
-    const int cluster_id = (int)blockIdx.x / CS;
-    // tj fastest: the tiles_n (= nb/256, e.g. 4) column tiles of one row panel are adjacent in launch order, so
-    // co-resident CTAs share every A row panel (and all share the few B panels) in L2 instead of each streaming
-    // its own A panel from DRAM (ncu, round 1: 8.1 GB DRAM reads per launch, 62 % L2 hit rate with ti fastest)
-    const int ctn = (g.tiles_n + CN - 1) / CN;            // cluster tiles along N
+    // cluster tiles: (CM * ROWS) x (CN * CTN); tj fastest, so co-resident CTAs share every A row panel in L2
+    const int ctn = (2 * g.tiles_n + CN - 1) / CN;
+    int cluster_id = (int)blockIdx.x / CS;
+    int seg = 0, tail_idx = 0;
+    const bool split = (g.nseg > 1 && cluster_id >= g.split_from);
+    if (split) {                                             // tail clusters: segment slowest
+        const int idx = cluster_id - g.split_from;
+        seg = idx / g.ntail; tail_idx = idx - seg * g.ntail;
+        cluster_id = g.split_from + tail_idx;
+    }
     const int ci = cluster_id / ctn, cj = cluster_id % ctn;
-    const int ti = ci * CM + cm, tj = cj * CN + cn;
-    const int64_t grow0 = g.row0 + (int64_t)ti * TM;      // global row of tile row 0
-    const int64_t gcol0 = g.col0 + (int64_t)tj * TN;      // global col of tile col 0
-    // cluster-uniform decisions
-    const int64_t crow_lo = g.row0 + (int64_t)ci * CM * TM, crow_hi = crow_lo + (int64_t)CM * TM - 1;
-    const int64_t ccol_lo = g.col0 + (int64_t)cj * CN * TN;
-    if (g.skip_upper && crow_hi < ccol_lo) return;        // every tile of the cluster lies above the diagonal
+    const int seg_k0 = g.k_begin + seg * g.kseg;             // first K column of this tile's segment
+    const int seg_K = split ? ((g.K - seg * g.kseg < g.kseg) ? (g.K - seg * g.kseg) : g.kseg) : g.K;
+    const int64_t crow_lo = g.row0 + (int64_t)ci * CM * ROWS, ccol_lo = g.col0 + (int64_t)cj * CN * CTN;
+    const int64_t grow0 = crow_lo + (int64_t)cm * ROWS;      // global row of this CTA's tile row 0
+    const int64_t gcol0 = ccol_lo + (int64_t)cn * CTN;       // global col of this CTA's tile col 0
+    // cluster-uniform decision
+    if (g.skip_upper && crow_lo + (int64_t)CM * ROWS - 1 < ccol_lo) return;   // every tile of the cluster lies above the diagonal
     // Pairs with s + t >= S are dropped everywhere.  Off the diagonal they are zero-mean; on the diagonal they
     // are sums of squares (a systematic bias), which cut_digits_kernel accumulates exactly per row and
     // diag_correct_kernel subtracts from C_ii -- so every tile does the same S(S+1)/2 products.
     const int S = g.S;
-    const int NG = S;
 
     uint16_t mask_a = 0, mask_b = 0;
 #pragma unroll
@@ -333,73 +340,64 @@ __global__ void __launch_bounds__(THREADS, 1) i8_update_kernel(const __grid_cons
     const uint16_t mask_all = mask_a | mask_b;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, CM + CN - 1); }
-        mbar_init(tfull + 0, 1); mbar_init(tfull + 1, 1);
-        mbar_init(tempty + 0, 4); mbar_init(tempty + 1, 4);
+        for (int s = 0; s < STAGES; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, 2 * (CM + CN - 1)); }
         *abort_flag = 0;
         asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
     }
-    if (warp == 1) {  // TMEM: all 512 columns (two 256-column int32 accumulators)
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;\n" ::"r"(smem_u32(tmem_ptr)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
     if (CS > 1) cluster_sync_all();   // mates' barriers must be initialised before any multicast lands
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
 
-    const int KT = g.K / KC;
-    const int64_t brow0 = g.b_row0 + (int64_t)tj * TN;  // global row of the B operand's first row
+    const int KT = seg_K / KC;
+    const int64_t brow0 = g.b_row0 + (gcol0 - g.col0);      // global row of the B operand's first row
 
     const bool prof = (g.dbg != nullptr);
     const long long t_cta0 = prof ? clock64() : 0;
-    if (warp == 0) {
+    if (warp == 8) {
         // ===== TMA producer =====
         if (lane == 0) {
             unsigned long long w_prod = 0;
             const long long t_role0 = prof ? clock64() : 0;
-            // one ring stage: (A plane s, B plane t) of K chunk kc
-            // one 128-byte x 64-row box of digit plane `pl` at K chunk kc into this CTA's (and its mates') current stage
-            const int kchunk0 = g.k_begin / KC;
+            const int kchunk0 = seg_k0 / KC;
             int stage = 0;
             uint32_t phase = 0;
             bool ok = true;
+            // one BOXR-row x 128-byte box of digit plane `pl` at K chunk kc into this CTA's (and its mates') current stage
             auto load_box = [&](uint8_t* dst, int kc, int row, int pl, bool mc, uint16_t mask) {
                 if (g.layout == 1) {
                     if (mc) tma_load_4d_mc(dst, &maps.all, full + stage, 0, pl, row, kchunk0 + kc, mask);
                     else tma_load_4d(dst, &maps.all, full + stage, 0, pl, row, kchunk0 + kc);
                 } else {
-                    if (mc) tma_load_3d_mc(dst, &maps.all, full + stage, g.k_begin + kc * KC, row, pl, mask);
-                    else tma_load_3d(dst, &maps.all, full + stage, g.k_begin + kc * KC, row, pl);
+                    if (mc) tma_load_3d_mc(dst, &maps.all, full + stage, seg_k0 + kc * KC, row, pl, mask);
+                    else tma_load_3d(dst, &maps.all, full + stage, seg_k0 + kc * KC, row, pl);
                 }
             };
+            // one ring stage: (A plane s, B plane t) of K chunk kc
             auto issue_stage = [&](int s, int t, int kc) {
-                        if (!mbar_wait_t(empty + stage, phase ^ 1, abort_flag, prof, w_prod)) { ok = false; return; }
-                        uint8_t* a_dst = smem + stage * STAGE_BYTES;
-                        uint8_t* b_dst = a_dst + A_BYTES;
-                        mbar_expect_tx(full + stage, STAGE_BYTES);   // own + mates' slices land on this barrier
-                        constexpr int A_ROWS = TM / CN, B_ROWS = TN / CM;
-                        if (g.prefetch > 0 && g.layout == 0 && kc + g.prefetch < KT) {   // own slices, `prefetch` K-chunks ahead, into L2
-                            const int kp = g.k_begin + (kc + g.prefetch) * KC;
+                if (!mbar_wait_t(empty + stage, phase ^ 1, abort_flag, prof, w_prod)) { ok = false; return; }
+                uint8_t* a_dst = smem + stage * STAGE_BYTES;
+                uint8_t* b_dst = a_dst + A_BYTES;
+                mbar_expect_tx(full + stage, STAGE_BYTES);   // own + mates' slices land on this barrier
+                constexpr int A_ROWS = ROWS / CN, B_ROWS = CTN / CM;
+                if (g.prefetch > 0 && g.layout == 0 && kc + g.prefetch < KT) {   // own slices, `prefetch` K-chunks ahead, into L2
+                    const int kp = seg_k0 + (kc + g.prefetch) * KC;
 #pragma unroll
-                            for (int bx = 0; bx < A_ROWS / BOXR; ++bx)
-                                tma_prefetch_3d(&maps.all, kp, (int)grow0 + cn * A_ROWS + bx * BOXR, s);
+                    for (int bx = 0; bx < A_ROWS / BOXR; ++bx)
+                        tma_prefetch_3d(&maps.all, kp, (int)grow0 + cn * A_ROWS + bx * BOXR, s);
 #pragma unroll
-                            for (int bx = 0; bx < B_ROWS / BOXR; ++bx)
-                                tma_prefetch_3d(&maps.all, kp, (int)brow0 + cm * B_ROWS + bx * BOXR, t);
-                        }
+                    for (int bx = 0; bx < B_ROWS / BOXR; ++bx)
+                        tma_prefetch_3d(&maps.all, kp, (int)brow0 + cm * B_ROWS + bx * BOXR, t);
+                }
 #pragma unroll
-                        for (int bx = 0; bx < A_ROWS / BOXR; ++bx) {
-                            const int r = cn * A_ROWS + bx * BOXR;
-                            load_box(a_dst + r * KC, kc, (int)grow0 + r, s, CN > 1, mask_a);
-                        }
+                for (int bx = 0; bx < A_ROWS / BOXR; ++bx) {
+                    const int r = cn * A_ROWS + bx * BOXR;
+                    load_box(a_dst + r * KC, kc, (int)grow0 + r, s, CN > 1, mask_a);
+                }
 #pragma unroll
-                        for (int bx = 0; bx < B_ROWS / BOXR; ++bx) {
-                            const int r = cm * B_ROWS + bx * BOXR;
-                            load_box(b_dst + r * KC, kc, (int)brow0 + r, t, CM > 1, mask_b);
-                        }
-                        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+                for (int bx = 0; bx < B_ROWS / BOXR; ++bx) {
+                    const int r = cm * B_ROWS + bx * BOXR;
+                    load_box(b_dst + r * KC, kc, (int)brow0 + r, t, CM > 1, mask_b);
+                }
+                if (++stage == STAGES) { stage = 0; phase ^= 1; }
             };
             if constexpr (PG) {
                 const int npass = g.pg_single ? S : (S + 1) / 2;
@@ -411,7 +409,7 @@ __global__ void __launch_bounds__(THREADS, 1) i8_update_kernel(const __grid_cons
                         for (int i = 0; i <= top && ok; ++i) issue_stage(i, top - i, kc);
                 }
             } else {
-                for (int gi = 0; gi < NG && ok; ++gi) {
+                for (int gi = 0; gi < S && ok; ++gi) {
                     const int s_lo = (gi - (S - 1) > 0) ? gi - (S - 1) : 0, s_hi = (gi < S - 1) ? gi : S - 1;
                     for (int s = s_lo; s <= s_hi && ok; ++s)
                         for (int kc = 0; kc < KT && ok; ++kc) issue_stage(s, gi - s, kc);
@@ -419,603 +417,140 @@ __global__ void __launch_bounds__(THREADS, 1) i8_update_kernel(const __grid_cons
             }
             if (prof) { dbg_add(g.dbg, DBG_PROD_WAIT, w_prod); dbg_add(g.dbg, DBG_PROD_TOTAL, (unsigned long long)(clock64() - t_role0)); }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer (one thread) =====
-        if (lane == 0) {
-            unsigned long long w_full = 0, w_tempty = 0;
-            const long long t_role0 = prof ? clock64() : 0;
-            int stage = 0;
-            uint32_t phase = 0;
-            bool ok = true;
-            if constexpr (PG) {
-                const int npass = g.pg_single ? S : (S + 1) / 2;
-                for (int P = 0; P < npass && ok; ++P) {
-                    int g0; bool two;
-                    pg_pass(S, g.pg_single, P, g0, two);
-                    const int top = two ? g0 + 1 : g0;
-                    if (P >= 1) {  // the epilogue must have drained both accumulators (pair P-1)
-                        if (!mbar_wait_t(tempty, (uint32_t)((P - 1) & 1), abort_flag, prof, w_tempty)) { ok = false; break; }
-                        tc_fence_after();
-                    }
-                    const uint32_t acc0 = tmem_base, acc1 = tmem_base + (uint32_t)TN;
-                    uint32_t accum0 = 0, accum1 = 0;
-                    for (int kc = 0; kc < KT && ok; ++kc) {
-                        uint32_t prev_a = 0;
-                        int prev_stage = 0;
-                        for (int i = 0; i <= top; ++i) {
-                            if (!mbar_wait_t(full + stage, phase, abort_flag, prof, w_full)) { ok = false; break; }
-                            tc_fence_after();
-                            const uint32_t a_addr = smem_u32(smem + stage * STAGE_BYTES);
-                            const uint32_t b_addr = a_addr + A_BYTES;
-                            if (two) {
-#pragma unroll
-                                for (int kk = 0; kk < KC / 32; ++kk) {   // A_i x B_{top-i}: group top
-                                    umma_i8(acc1, make_desc(a_addr + kk * 32), make_desc(b_addr + kk * 32), accum1);
-                                    accum1 = 1;
-                                }
-                                if (i >= 1) {
-#pragma unroll
-                                    for (int kk = 0; kk < KC / 32; ++kk) {   // A_{i-1} x B_{top-i}: group top - 1
-                                        umma_i8(acc0, make_desc(prev_a + kk * 32), make_desc(b_addr + kk * 32), accum0);
-                                        accum0 = 1;
-                                    }
-                                    // stage i-1 is now dead: its A was just used for the last time, its B one step ago
-                                    if (CS > 1) tc_commit_mc(empty + prev_stage, mask_all); else tc_commit(empty + prev_stage);
-                                }
-                                if (i == top) { if (CS > 1) tc_commit_mc(empty + stage, mask_all); else tc_commit(empty + stage); }
-                            } else {
-#pragma unroll
-                                for (int kk = 0; kk < KC / 32; ++kk) {
-                                    umma_i8(acc0, make_desc(a_addr + kk * 32), make_desc(b_addr + kk * 32), accum0);
-                                    accum0 = 1;
-                                }
-                                if (CS > 1) tc_commit_mc(empty + stage, mask_all); else tc_commit(empty + stage);
-                            }
-                            prev_a = a_addr;
-                            prev_stage = stage;
-                            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-                        }
-                    }
-                    if (ok) tc_commit(tfull);    // both accumulators of pair P complete
-                }
-            } else {
-                for (int gi = 0; gi < NG && ok; ++gi) {
-                    const int acc = gi & 1;
-                    if (gi >= 2) {  // the epilogue must have drained this accumulator (group gi-2)
-                        if (!mbar_wait_t(tempty + acc, ((gi >> 1) - 1) & 1, abort_flag, prof, w_tempty)) { ok = false; break; }
-                        tc_fence_after();
-                    }
-                    const uint32_t tacc = tmem_base + (uint32_t)acc * TN;
-                    uint32_t accumulate = 0;
-                    const int s_lo = (gi - (S - 1) > 0) ? gi - (S - 1) : 0, s_hi = (gi < S - 1) ? gi : S - 1;
-                    for (int s = s_lo; s <= s_hi && ok; ++s) {
-                        for (int kc = 0; kc < KT; ++kc) {
-                            if (!mbar_wait_t(full + stage, phase, abort_flag, prof, w_full)) { ok = false; break; }
-                            tc_fence_after();
-                            const uint32_t a_addr = smem_u32(smem + stage * STAGE_BYTES);
-                            const uint32_t b_addr = a_addr + A_BYTES;
-#pragma unroll
-                            for (int kk = 0; kk < KC / 32; ++kk) {
-                                umma_i8(tacc, make_desc(a_addr + kk * 32), make_desc(b_addr + kk * 32), accumulate);
-                                accumulate = 1;
-                            }
-                            // free the slot in every CTA whose producer writes into it (row- and column-mates)
-                            if (CS > 1) tc_commit_mc(empty + stage, mask_all); else tc_commit(empty + stage);
-                            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-                        }
-                    }
-                    if (ok) tc_commit(tfull + acc);    // accumulator of group gi complete
-                }
-            }
-            if (prof) {
-                dbg_add(g.dbg, DBG_MMA_WAIT_FULL, w_full); dbg_add(g.dbg, DBG_MMA_WAIT_TEMPTY, w_tempty);
-                dbg_add(g.dbg, DBG_MMA_TOTAL, (unsigned long long)(clock64() - t_role0));
-            }
-        }
     } else {
-        // ===== epilogue warps 2..5: TMEM lane quarter = warp % 4 =====
-        unsigned long long w_tfull = 0;
-        const long long t_role0 = prof ? clock64() : 0;
-        const int q = warp & 3;
-        const int row = q * 32 + lane;            // tile row owned by this thread
-        const int64_t gr = grow0 + row;
-        const bool row_ok = gr < g.n_rows;        // padding tiles of an incomplete cluster do no stores
-        const double rsi = row_ok ? g.rs[gr] : 0.0;
-        double* crow = g.C + (row_ok ? gr : 0) * g.ldc;
+        // ===== consumer warpgroup wg: wgmma on rows [wg * 64 MW, (wg + 1) * 64 MW) of the tile, then the fp64 epilogue =====
+        const int wg = warp >> 2, wl = threadIdx.x & 127;
+        const bool leader = (wl == 0);
+        const bool prof_wg = prof && wg == 0 && leader;
+        unsigned long long w_full = 0, t_epi = 0;
+        const long long t_role0 = prof_wg ? clock64() : 0;
+        // this thread's rows (two per m64 block) and the first of its columns
+        const int rloc = wg * 64 * MW + 16 * (wl >> 5) + ((wl & 31) >> 2);
+        const int64_t gc_lane = gcol0 + 2 * (lane & 3);
+        double* crow[MW][2];
+        bool rok[MW][2];
+        double rsi[MW][2];
+#pragma unroll
+        for (int mw = 0; mw < MW; ++mw)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int lr = rloc + 64 * mw + 8 * h;
+                const int64_t gr = grow0 + lr;
+                rok[mw][h] = gr < g.n_rows;           // padding tiles of an incomplete cluster do no stores
+                rsi[mw][h] = rok[mw][h] ? g.rs[gr] : 0.0;
+                // segment >= 1: this cluster's scratch tile, addressed like C through a virtual base (columns are GLOBAL indices)
+                crow[mw][h] = (seg == 0) ? g.C + (rok[mw][h] ? gr : 0) * g.ldc
+                                         : g.Cseg + ((int64_t)(seg - 1) * g.ntail + tail_idx) * ((int64_t)CM * ROWS * CN * CTN)
+                                               + (gr - crow_lo) * (CN * CTN) - ccol_lo;
+            }
+        // release a stage in every CTA whose producer writes into it (row- and column-mates, this CTA included)
+        auto release = [&](int st) {
+            if (!leader) return;
+            if (CS == 1) { mbar_arrive(empty + st); return; }
+            const uint32_t local = smem_u32(empty + st);
+#pragma unroll
+            for (int r = 0; r < CS; ++r)
+                if ((mask_all >> r) & 1) mbar_arrive_cluster(mapa(local, (uint32_t)r));
+        };
+        uint32_t acc0[MW][64], acc1[64];
+#pragma unroll
+        for (int i = 0; i < 64; ++i) {
+            acc1[i] = 0;
+#pragma unroll
+            for (int mw = 0; mw < MW; ++mw) acc0[mw][i] = 0;
+        }
+        int stage = 0;
+        uint32_t phase = 0;
         bool ok = true;
+        const uint32_t a_off = (uint32_t)(wg * 64 * MW * KC);
         if constexpr (PG) {
             const int npass = g.pg_single ? S : (S + 1) / 2;
             for (int P = 0; P < npass && ok; ++P) {
                 int g0; bool two;
                 pg_pass(S, g.pg_single, P, g0, two);
-                if (!mbar_wait_t(tfull, (uint32_t)(P & 1), abort_flag, prof, w_tfull)) { ok = false; break; }
-                tc_fence_after();
+                const int top = two ? g0 + 1 : g0;
+                uint32_t accum0 = 0, accum1 = 0;
+                for (int kc = 0; kc < KT && ok; ++kc) {
+                    uint32_t prev_a = 0;
+                    int prev_stage = 0;
+                    for (int i = 0; i <= top; ++i) {
+                        if (!mbar_wait_t(full + stage, phase, abort_flag, prof_wg, w_full)) { ok = false; break; }
+                        const uint32_t a_addr = smem_u32(smem + stage * STAGE_BYTES) + a_off;
+                        const uint32_t b_addr = smem_u32(smem + stage * STAGE_BYTES + A_BYTES);
+                        wg_fence();
+                        if (two) {
+                            mma_stage(acc1, a_addr, b_addr, accum1);                        // A_i x B_{top-i}: group top
+                            if (i >= 1) mma_stage(acc0[0], prev_a, b_addr, accum0);         // A_{i-1} x B_{top-i}: group top - 1
+                            wg_commit();
+                            wg_wait0();
+                            // stage i-1 is now dead: its A was just used for the last time, its B one step ago
+                            if (i >= 1) release(prev_stage);
+                            if (i == top) release(stage);
+                        } else {
+                            mma_stage(acc0[0], a_addr, b_addr, accum0);
+                            wg_commit();
+                            wg_wait0();
+                            release(stage);
+                        }
+                        prev_a = a_addr;
+                        prev_stage = stage;
+                        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+                    }
+                }
+                if (!ok) break;
                 // group g0 weighs 2^-(12 + 7 g0); group g0 + 1 is 2^-7 of that.  a0 + a1 2^-7 is exact in fp64
                 // (|a| < 2^31), so the pair costs ONE rounding and one read-modify-write of the fp64 tile.
-                const double wg = __longlong_as_double((long long)(1023 - (12 + 7 * g0)) << 52);
-                const double sc = -(rsi * wg);
-                {
-                    const uint32_t trow = tmem_base + ((uint32_t)(q * 32) << 16);
-                    if (two) epi_rmw_row<true>(trow, trow + (uint32_t)TN, crow, g.rs, gcol0, g.n_rows, row_ok, sc);
-                    else epi_rmw_row<false>(trow, trow, crow, g.rs, gcol0, g.n_rows, row_ok, sc);
-                }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(tempty);
+                const long long te0 = prof_wg ? clock64() : 0;
+                const double wgt = __longlong_as_double((long long)(1023 - (12 + 7 * g0)) << 52);
+                const double sc0 = -(rsi[0][0] * wgt), sc1 = -(rsi[0][1] * wgt);
+                if (two) epi_rmw<true>(acc0[0], acc1, crow[0][0], crow[0][1], g.rs, gc_lane, g.n_rows, rok[0][0], rok[0][1], sc0, sc1);
+                else epi_rmw<false>(acc0[0], acc0[0], crow[0][0], crow[0][1], g.rs, gc_lane, g.n_rows, rok[0][0], rok[0][1], sc0, sc1);
+                if (prof_wg) t_epi += (unsigned long long)(clock64() - te0);
             }
         } else {
-            for (int gi = 0; gi < NG && ok; ++gi) {
-                const int acc = gi & 1;
-                if (!mbar_wait_t(tfull + acc, (gi >> 1) & 1, abort_flag, prof, w_tfull)) { ok = false; break; }
-                tc_fence_after();
-                // weight 2^-(12 + 7 gi), exact power of two
-                const double wg = __longlong_as_double((long long)(1023 - (12 + 7 * gi)) << 52);
-                const double sc = -(rsi * wg);
-                {
-                    const uint32_t trow = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * TN);
-                    epi_rmw_row<false>(trow, trow, crow, g.rs, gcol0, g.n_rows, row_ok, sc);
+            for (int gi = 0; gi < S && ok; ++gi) {
+                uint32_t accumulate = 0;
+                const int s_lo = (gi - (S - 1) > 0) ? gi - (S - 1) : 0, s_hi = (gi < S - 1) ? gi : S - 1;
+                for (int s = s_lo; s <= s_hi && ok; ++s) {
+                    for (int kc = 0; kc < KT; ++kc) {
+                        if (!mbar_wait_t(full + stage, phase, abort_flag, prof_wg, w_full)) { ok = false; break; }
+                        const uint32_t a_addr = smem_u32(smem + stage * STAGE_BYTES) + a_off;
+                        const uint32_t b_addr = smem_u32(smem + stage * STAGE_BYTES + A_BYTES);
+                        wg_fence();
+#pragma unroll
+                        for (int mw = 0; mw < MW; ++mw) {
+                            uint32_t acc_flag = accumulate;
+                            mma_stage(acc0[mw], a_addr + (uint32_t)(mw * 64 * KC), b_addr, acc_flag);
+                        }
+                        accumulate = 1;
+                        wg_commit();
+                        wg_wait0();
+                        release(stage);
+                        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+                    }
                 }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(tempty + acc);
+                if (!ok) break;
+                const long long te0 = prof_wg ? clock64() : 0;
+                // weight 2^-(12 + 7 gi), exact power of two
+                const double wgt = __longlong_as_double((long long)(1023 - (12 + 7 * gi)) << 52);
+#pragma unroll
+                for (int mw = 0; mw < MW; ++mw)
+                    epi_rmw<false>(acc0[mw], acc0[mw], crow[mw][0], crow[mw][1], g.rs, gc_lane, g.n_rows, rok[mw][0], rok[mw][1],
+                                   -(rsi[mw][0] * wgt), -(rsi[mw][1] * wgt));
+                if (prof_wg) t_epi += (unsigned long long)(clock64() - te0);
             }
         }
-        if (prof && warp == 2 && lane == 0) {
-            dbg_add(g.dbg, DBG_EPI_WAIT_TFULL, w_tfull);
-            dbg_add(g.dbg, DBG_EPI_TOTAL, (unsigned long long)(clock64() - t_role0));
+        if (prof_wg) {
+            dbg_add(g.dbg, DBG_MMA_WAIT_FULL, w_full);
+            dbg_add(g.dbg, DBG_EPI_TOTAL, t_epi);
+            dbg_add(g.dbg, DBG_MMA_TOTAL, (unsigned long long)(clock64() - t_role0));
         }
     }
 
-    tc_fence_before();
     __syncthreads();
     if (CS > 1) cluster_sync_all();   // no CTA may exit while mates still multicast into it / arrive on its barriers
     if (prof && threadIdx.x == 0) { dbg_add(g.dbg, DBG_CTAS, 1ull); dbg_add(g.dbg, DBG_CTA_TOTAL, (unsigned long long)(clock64() - t_cta0)); }
     if (threadIdx.x == 0 && *abort_flag) atomicExch(g.error_flag, 1);
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;\n" ::"r"(tmem_base) : "memory");
-    }
-}
-
-// ---- 2-SM variant: tcgen05.mma.cta_group::2, one 256 x 256 tile per CTA pair -------------------------------
-// Each CTA of the pair fetches its own 128 A rows and only HALF of the B tile (128 of 256 rows); the MMA reads
-// the other half from the peer's shared memory.  Per-SM operand ingest drops from 48 KB to 32 KB per K = 128
-// stage, which is what bounds the 1-SM kernel (ncu: tensor pipe ~50 % with nothing else saturated), and the
-// freed shared memory buys two more pipeline stages.
-constexpr int STAGES2 = 6;
-constexpr int STAGE2_BYTES = A_BYTES + A_BYTES;             // A 128 rows + B half 128 rows = 32 KiB
-constexpr int SMEM2_BYTES = STAGES2 * STAGE2_BYTES + 1024 + 256;
-constexpr uint32_t IDESC2 = (2u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(TN >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-
-__device__ __forceinline__ uint32_t mapa_rank0(uint32_t local_addr) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, 0;\n" : "=r"(r) : "r"(local_addr));
-    return r;
-}
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const CUtensorMap* map, uint32_t leader_bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];\n" ::"r"(
-            smem_u32(smem_dst)),
-        "l"(map), "r"(leader_bar), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_2sm(void* smem_dst, const CUtensorMap* map, uint32_t leader_bar, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];\n" ::"r"(
-            smem_u32(smem_dst)),
-        "l"(map), "r"(leader_bar), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
-__device__ __forceinline__ void umma_i8_2sm(uint32_t tmem_c, uint64_t da, uint64_t db, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::i8 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_c),
-        "l"(da), "l"(db), "r"(IDESC2), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void tc_commit_2sm(uint64_t* bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n" ::"r"(
-                     smem_u32(bar)),
-                 "h"(mask)
-                 : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];\n" ::"r"(cluster_addr) : "memory");
-}
-
-// PG: paired digit groups as in i8_update_kernel<.., true> (one ring stage = (A plane i, B-half plane top - i) feeds
-// group top with A_i and group top - 1 with the previous stage's A): per SM and pair product 21.7 KB from L2 / 19 KB
-// written to shared memory instead of 48 / 48 for the unpaired 1-SM loop, and the operand reads of the tensor core drop
-// from 96 to 64 B/clk -- shared-memory bandwidth (TMA writes + UMMA reads against 128 B/clk/SM) stops being a bound.
-template <bool PG>
-__global__ void __launch_bounds__(THREADS, 1) i8_update_kernel_2sm(const __grid_constant__ Maps maps, const Args g) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES2 * STAGE2_BYTES);
-    uint64_t* full = bars;                     // [STAGES2]  (used in the leader CTA only)
-    uint64_t* empty = bars + STAGES2;          // [STAGES2]  (one per CTA, signalled by the MMA commit multicast)
-    uint64_t* tfull = bars + 2 * STAGES2;      // [2]        (one per CTA)
-    uint64_t* tempty = bars + 2 * STAGES2 + 2; // [2]        (leader only; 8 arrivals: 4 epilogue warps x 2 CTAs)
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * STAGES2 + 4);
-    volatile int* abort_flag = reinterpret_cast<volatile int*>(tmem_ptr + 1);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    int crank;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;\n" : "=r"(crank));
-    const bool leader = (crank == 0);
-    int pair_id = (int)blockIdx.x >> 1;
-    const int ptm = (g.tiles_m + 1) / 2;                     // row pairs
-    int seg = 0, tail_idx = 0;
-    const bool split = (g.nseg > 1 && pair_id >= g.split_from);
-    if (split) {                                             // tail tiles: segment slowest
-        const int idx = pair_id - g.split_from;
-        seg = idx / g.ntail; tail_idx = idx - seg * g.ntail;
-        pair_id = g.split_from + tail_idx;
-    }
-    (void)ptm;
-    const int pi = pair_id / g.tiles_n, tj = pair_id % g.tiles_n;   // tj fastest (L2 sharing of A panels)
-    const int seg_k0 = g.k_begin + seg * g.kseg;             // first K column of this tile's segment
-    const int seg_K = split ? ((g.K - seg * g.kseg < g.kseg) ? (g.K - seg * g.kseg) : g.kseg) : g.K;
-    const int64_t prow0 = g.row0 + (int64_t)pi * 2 * TM;     // first row of the 256-row pair tile
-    const int64_t grow0 = prow0 + (int64_t)crank * TM;       // this CTA's 128 rows
-    const int64_t gcol0 = g.col0 + (int64_t)tj * TN;
-    if (g.skip_upper && prow0 + 2 * TM - 1 < gcol0) return;  // pair-uniform
-
-    const int S = g.S;
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES2; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, 1); }
-        mbar_init(tfull + 0, 1); mbar_init(tfull + 1, 1);
-        mbar_init(tempty + 0, 8); mbar_init(tempty + 1, 8);
-        *abort_flag = 0;
-        asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], 512;\n" ::"r"(smem_u32(tmem_ptr)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;\n" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
-
-    const int KT = seg_K / KC;
-    const int64_t brow0 = g.b_row0 + (int64_t)tj * TN + (int64_t)crank * 128;  // this CTA's half of the B rows
-
-    const bool prof = (g.dbg != nullptr);
-    const long long t_cta0 = prof ? clock64() : 0;
-    if (warp == 0) {
-        // ===== TMA producer (both CTAs; completion is signalled on the LEADER's full barrier) =====
-        if (lane == 0) {
-            unsigned long long w_prod = 0;
-            const long long t_role0 = prof ? clock64() : 0;
-            int stage = 0;
-            uint32_t phase = 0;
-            bool ok = true;
-            if constexpr (PG) {
-                const int npass = g.pg_single ? S : (S + 1) / 2;
-                for (int P = 0; P < npass && ok; ++P) {
-                    int g0; bool two;
-                    pg_pass(S, g.pg_single, P, g0, two);
-                    const int top = two ? g0 + 1 : g0;
-                    for (int kc = 0; kc < KT && ok; ++kc)
-                        for (int i = 0; i <= top; ++i) {     // stage i: (A plane i, B-half plane top - i), one 3-D map
-                            if (!mbar_wait_t(empty + stage, phase ^ 1, abort_flag, prof, w_prod)) { ok = false; break; }
-                            uint8_t* a_dst = smem + stage * STAGE2_BYTES;
-                            uint8_t* b_dst = a_dst + A_BYTES;
-                            if (leader) mbar_expect_tx(full + stage, 2 * STAGE2_BYTES);
-                            const uint32_t lbar = mapa_rank0(smem_u32(full + stage));
-                            const int kx = seg_k0 + kc * KC;
-#pragma unroll
-                            for (int bx = 0; bx < TM / BOXR; ++bx) {
-                                tma_load_3d_2sm(a_dst + bx * BOXR * KC, &maps.all, lbar, kx, (int)grow0 + bx * BOXR, i);
-                                tma_load_3d_2sm(b_dst + bx * BOXR * KC, &maps.all, lbar, kx, (int)brow0 + bx * BOXR, top - i);
-                            }
-                            if (++stage == STAGES2) { stage = 0; phase ^= 1; }
-                        }
-                }
-            } else {
-            for (int gi = 0; gi < S && ok; ++gi) {
-                for (int s = 0; s <= gi && ok; ++s) {
-                    const int t = gi - s;
-                    for (int kc = 0; kc < KT; ++kc) {
-                        if (!mbar_wait_t(empty + stage, phase ^ 1, abort_flag, prof, w_prod)) { ok = false; break; }
-                        uint8_t* a_dst = smem + stage * STAGE2_BYTES;
-                        uint8_t* b_dst = a_dst + A_BYTES;
-                        if (leader) mbar_expect_tx(full + stage, 2 * STAGE2_BYTES);   // both CTAs' bytes
-                        const uint32_t lbar = mapa_rank0(smem_u32(full + stage));
-                        const int kx = seg_k0 + kc * KC;
-#pragma unroll
-                        for (int bx = 0; bx < TM / BOXR; ++bx) {
-                            tma_load_3d_2sm(a_dst + bx * BOXR * KC, &maps.all, lbar, kx, (int)grow0 + bx * BOXR, s);
-                            tma_load_3d_2sm(b_dst + bx * BOXR * KC, &maps.all, lbar, kx, (int)brow0 + bx * BOXR, t);
-                        }
-                        if (++stage == STAGES2) { stage = 0; phase ^= 1; }
-                    }
-                }
-            }
-            }
-            if (prof && leader) { dbg_add(g.dbg, DBG_PROD_WAIT, w_prod); dbg_add(g.dbg, DBG_PROD_TOTAL, (unsigned long long)(clock64() - t_role0)); }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer: one thread of the leader CTA drives both SMs =====
-        if (leader && lane == 0) {
-            unsigned long long w_full = 0, w_tempty = 0;
-            const long long t_role0 = prof ? clock64() : 0;
-            int stage = 0;
-            uint32_t phase = 0;
-            bool ok = true;
-            if constexpr (PG) {
-                const int npass = g.pg_single ? S : (S + 1) / 2;
-                for (int P = 0; P < npass && ok; ++P) {
-                    int g0; bool two;
-                    pg_pass(S, g.pg_single, P, g0, two);
-                    const int top = two ? g0 + 1 : g0;
-                    if (P >= 1) {   // both accumulators drained by the epilogue of pass P-1 (8 arrivals: 4 warps x 2 CTAs)
-                        if (!mbar_wait_t(tempty, (uint32_t)((P - 1) & 1), abort_flag, prof, w_tempty)) { ok = false; break; }
-                        tc_fence_after();
-                    }
-                    const uint32_t acc0 = tmem_base, acc1 = tmem_base + (uint32_t)TN;
-                    uint32_t accum0 = 0, accum1 = 0;
-                    for (int kc = 0; kc < KT && ok; ++kc) {
-                        uint32_t prev_a = 0;
-                        int prev_stage = 0;
-                        for (int i = 0; i <= top; ++i) {
-                            if (!mbar_wait_t(full + stage, phase, abort_flag, prof, w_full)) { ok = false; break; }
-                            tc_fence_after();
-                            const uint32_t a_addr = smem_u32(smem + stage * STAGE2_BYTES);
-                            const uint32_t b_addr = a_addr + A_BYTES;
-                            if (two) {
-#pragma unroll
-                                for (int kk = 0; kk < KC / 32; ++kk) {   // A_i x B_{top-i}: group top
-                                    umma_i8_2sm(acc1, make_desc(a_addr + kk * 32), make_desc(b_addr + kk * 32), accum1);
-                                    accum1 = 1;
-                                }
-                                if (i >= 1) {
-#pragma unroll
-                                    for (int kk = 0; kk < KC / 32; ++kk) {   // A_{i-1} x B_{top-i}: group top - 1
-                                        umma_i8_2sm(acc0, make_desc(prev_a + kk * 32), make_desc(b_addr + kk * 32), accum0);
-                                        accum0 = 1;
-                                    }
-                                    tc_commit_2sm(empty + prev_stage, 0x3);   // stage i-1 is dead in both CTAs
-                                }
-                                if (i == top) tc_commit_2sm(empty + stage, 0x3);
-                            } else {
-#pragma unroll
-                                for (int kk = 0; kk < KC / 32; ++kk) {
-                                    umma_i8_2sm(acc0, make_desc(a_addr + kk * 32), make_desc(b_addr + kk * 32), accum0);
-                                    accum0 = 1;
-                                }
-                                tc_commit_2sm(empty + stage, 0x3);
-                            }
-                            prev_a = a_addr;
-                            prev_stage = stage;
-                            if (++stage == STAGES2) { stage = 0; phase ^= 1; }
-                        }
-                    }
-                    if (ok) tc_commit_2sm(tfull, 0x3);    // both accumulators (in both CTAs) of pass P complete
-                }
-            } else
-            for (int gi = 0; gi < S && ok; ++gi) {
-                const int acc = gi & 1;
-                if (gi >= 2) {
-                    if (!mbar_wait_t(tempty + acc, ((gi >> 1) - 1) & 1, abort_flag, prof, w_tempty)) { ok = false; break; }
-                    tc_fence_after();
-                }
-                const uint32_t tacc = tmem_base + (uint32_t)acc * TN;
-                uint32_t accumulate = 0;
-                for (int s = 0; s <= gi && ok; ++s) {
-                    for (int kc = 0; kc < KT; ++kc) {
-                        if (!mbar_wait_t(full + stage, phase, abort_flag, prof, w_full)) { ok = false; break; }
-                        tc_fence_after();
-                        const uint32_t a_addr = smem_u32(smem + stage * STAGE2_BYTES);
-                        const uint32_t b_addr = a_addr + A_BYTES;
-#pragma unroll
-                        for (int kk = 0; kk < KC / 32; ++kk) {
-                            umma_i8_2sm(tacc, make_desc(a_addr + kk * 32), make_desc(b_addr + kk * 32), accumulate);
-                            accumulate = 1;
-                        }
-                        tc_commit_2sm(empty + stage, 0x3);   // free the slot in both CTAs
-                        if (++stage == STAGES2) { stage = 0; phase ^= 1; }
-                    }
-                }
-                if (ok) tc_commit_2sm(tfull + acc, 0x3);     // accumulators (both CTAs) of group gi complete
-            }
-            if (prof) {
-                dbg_add(g.dbg, DBG_MMA_WAIT_FULL, w_full); dbg_add(g.dbg, DBG_MMA_WAIT_TEMPTY, w_tempty);
-                dbg_add(g.dbg, DBG_MMA_TOTAL, (unsigned long long)(clock64() - t_role0));
-            }
-        }
-    } else {
-        // ===== epilogue (both CTAs): this CTA's 128 rows x 256 columns =====
-        unsigned long long w_tfull = 0;
-        const long long t_role0 = prof ? clock64() : 0;
-        const int q = warp & 3;
-        const int row = q * 32 + lane;
-        const int64_t gr = grow0 + row;
-        const bool row_ok = gr < g.n_rows;
-        const double rsi = row_ok ? g.rs[gr] : 0.0;
-        // segment >= 1: this pair's scratch tile, addressed like C through a virtual base (columns are GLOBAL indices)
-        double* crow = (seg == 0) ? g.C + (row_ok ? gr : 0) * g.ldc
-                                   : g.Cseg + ((int64_t)(seg - 1) * g.ntail + tail_idx) * (2 * TM * TN)
-                                         + (int64_t)(crank * TM + row) * TN - gcol0;
-        const uint32_t tempty_leader0 = mapa_rank0(smem_u32(tempty + 0));
-        const uint32_t tempty_leader1 = mapa_rank0(smem_u32(tempty + 1));
-        bool ok = true;
-        if constexpr (PG) {
-            const int npass = g.pg_single ? S : (S + 1) / 2;
-            for (int P = 0; P < npass && ok; ++P) {
-                int g0; bool two;
-                pg_pass(S, g.pg_single, P, g0, two);
-                if (!mbar_wait_t(tfull, (uint32_t)(P & 1), abort_flag, prof, w_tfull)) { ok = false; break; }
-                tc_fence_after();
-                const double wg = __longlong_as_double((long long)(1023 - (12 + 7 * g0)) << 52);
-                const double sc = -(rsi * wg);
-                {
-                    const uint32_t trow = tmem_base + ((uint32_t)(q * 32) << 16);
-                    if (two) epi_rmw_row<true>(trow, trow + (uint32_t)TN, crow, g.rs, gcol0, g.n_rows, row_ok, sc);
-                    else epi_rmw_row<false>(trow, trow, crow, g.rs, gcol0, g.n_rows, row_ok, sc);
-                }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive_cluster(tempty_leader0);
-            }
-        } else
-        for (int gi = 0; gi < S && ok; ++gi) {
-            const int acc = gi & 1;
-            if (!mbar_wait_t(tfull + acc, (gi >> 1) & 1, abort_flag, prof, w_tfull)) { ok = false; break; }
-            tc_fence_after();
-            const double wg = __longlong_as_double((long long)(1023 - (12 + 7 * gi)) << 52);
-            const double sc = -(rsi * wg);
-            {
-                const uint32_t trow = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * TN);
-                epi_rmw_row<false>(trow, trow, crow, g.rs, gcol0, g.n_rows, row_ok, sc);
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(acc ? tempty_leader1 : tempty_leader0);
-        }
-        if (prof && leader && warp == 2 && lane == 0) {
-            dbg_add(g.dbg, DBG_EPI_WAIT_TFULL, w_tfull);
-            dbg_add(g.dbg, DBG_EPI_TOTAL, (unsigned long long)(clock64() - t_role0));
-        }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    if (prof && leader && threadIdx.x == 0) { dbg_add(g.dbg, DBG_CTAS, 1ull); dbg_add(g.dbg, DBG_CTA_TOTAL, (unsigned long long)(clock64() - t_cta0)); }
-    if (threadIdx.x == 0 && *abort_flag) atomicExch(g.error_flag, 1);
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, 512;\n" ::"r"(tmem_base) : "memory");
-    }
-}
-
-// ---- wide-tile variant: one CTA computes 256 x 256 (two M = 128 MMAs share every B stage) -------------------
-// Same per-SM operand ingest as the 2-SM pair kernel (64 KB per 2 x 128x256x128 MACs instead of 48 KB per one)
-// without a cluster.  TMEM holds the two 256-column accumulators of ONE digit group, so the epilogue of group g
-// is not overlapped with the MMAs of group g+1 (negligible once K is a few thousand).
-constexpr int STAGES_W = 3;
-constexpr int STAGE_W_BYTES = 2 * A_BYTES + B_BYTES;        // 64 KiB
-constexpr int SMEM_W_BYTES = STAGES_W * STAGE_W_BYTES + 1024 + 256;
-constexpr int THREADS_W = 320;                               // producer warp, MMA warp, 8 epilogue warps
-
-__global__ void __launch_bounds__(THREADS_W, 1) i8_update_kernel_wide(const __grid_constant__ Maps maps, const Args g) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES_W * STAGE_W_BYTES);
-    uint64_t* full = bars;                    // [STAGES_W]
-    uint64_t* empty = bars + STAGES_W;        // [STAGES_W]
-    uint64_t* tfull = bars + 2 * STAGES_W;    // [1]
-    uint64_t* tempty = bars + 2 * STAGES_W + 1;  // [1], 8 arrivals
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * STAGES_W + 2);
-    volatile int* abort_flag = reinterpret_cast<volatile int*>(tmem_ptr + 1);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int pi = (int)blockIdx.x / g.tiles_n, tj = (int)blockIdx.x % g.tiles_n;   // tj fastest
-    const int64_t prow0 = g.row0 + (int64_t)pi * 2 * TM;
-    const int64_t gcol0 = g.col0 + (int64_t)tj * TN;
-    if (g.skip_upper && prow0 + 2 * TM - 1 < gcol0) return;
-    const int S = g.S;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES_W; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, 1); }
-        mbar_init(tfull, 1);
-        mbar_init(tempty, 8);
-        *abort_flag = 0;
-        asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;\n" ::"r"(smem_u32(tmem_ptr)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
-    const int KT = g.K / KC;
-    const int64_t brow0 = g.b_row0 + (int64_t)tj * TN;
-
-    if (warp == 0) {
-        if (lane == 0) {
-            int stage = 0;
-            uint32_t phase = 0;
-            bool ok = true;
-            for (int gi = 0; gi < S && ok; ++gi)
-                for (int s = 0; s <= gi && ok; ++s) {
-                    const int t = gi - s;
-                    for (int kc = 0; kc < KT; ++kc) {
-                        if (!mbar_wait(empty + stage, phase ^ 1, abort_flag)) { ok = false; break; }
-                        uint8_t* a_dst = smem + stage * STAGE_W_BYTES;
-                        uint8_t* b_dst = a_dst + 2 * A_BYTES;
-                        mbar_expect_tx(full + stage, STAGE_W_BYTES);
-                        const int kx = g.k_begin + kc * KC;
-#pragma unroll
-                        for (int bx = 0; bx < (2 * TM) / BOXR; ++bx)
-                            tma_load_2d(a_dst + bx * BOXR * KC, &maps.plane[s], full + stage, kx, (int)prow0 + bx * BOXR);
-#pragma unroll
-                        for (int bx = 0; bx < TN / BOXR; ++bx)
-                            tma_load_2d(b_dst + bx * BOXR * KC, &maps.plane[t], full + stage, kx, (int)brow0 + bx * BOXR);
-                        if (++stage == STAGES_W) { stage = 0; phase ^= 1; }
-                    }
-                }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            int stage = 0;
-            uint32_t phase = 0;
-            bool ok = true;
-            for (int gi = 0; gi < S && ok; ++gi) {
-                if (gi >= 1) {  // both accumulators must have been drained (group gi-1)
-                    if (!mbar_wait(tempty, (gi - 1) & 1, abort_flag)) { ok = false; break; }
-                    tc_fence_after();
-                }
-                uint32_t accumulate = 0;
-                for (int s = 0; s <= gi && ok; ++s)
-                    for (int kc = 0; kc < KT; ++kc) {
-                        if (!mbar_wait(full + stage, phase, abort_flag)) { ok = false; break; }
-                        tc_fence_after();
-                        const uint32_t a0 = smem_u32(smem + stage * STAGE_W_BYTES);
-                        const uint32_t a1 = a0 + A_BYTES, b = a0 + 2 * A_BYTES;
-#pragma unroll
-                        for (int kk = 0; kk < KC / 32; ++kk) {
-                            const uint64_t db = make_desc(b + kk * 32);
-                            umma_i8(tmem_base, make_desc(a0 + kk * 32), db, accumulate);
-                            umma_i8(tmem_base + TN, make_desc(a1 + kk * 32), db, accumulate);
-                            accumulate = 1;
-                        }
-                        tc_commit(empty + stage);
-                        if (++stage == STAGES_W) { stage = 0; phase ^= 1; }
-                    }
-                if (ok) tc_commit(tfull);
-            }
-        }
-    } else {
-        const int q = warp & 3;
-        const int half = (warp >= 6) ? 1 : 0;                 // which 128-row sub-tile / accumulator
-        const int64_t gr = prow0 + half * TM + q * 32 + lane;
-        const bool row_ok = gr < g.n_rows;
-        const double rsi = row_ok ? g.rs[gr] : 0.0;
-        double* crow = g.C + (row_ok ? gr : 0) * g.ldc;
-        bool ok = true;
-        for (int gi = 0; gi < S && ok; ++gi) {
-            if (!mbar_wait(tfull, gi & 1, abort_flag)) { ok = false; break; }
-            tc_fence_after();
-            const double wg = __longlong_as_double((long long)(1023 - (12 + 7 * gi)) << 52);
-            const double sc = -(rsi * wg);
-            {
-                const uint32_t trow = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(half * TN);
-                epi_rmw_row<false>(trow, trow, crow, g.rs, gcol0, g.n_rows, row_ok, sc);
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tempty);
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (threadIdx.x == 0 && *abort_flag) atomicExch(g.error_flag, 1);
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;\n" ::"r"(tmem_base) : "memory");
 }
 
 // ---- digit cutting -------------------------------------------------------------------------------
@@ -1023,8 +558,7 @@ __global__ void __launch_bounds__(THREADS_W, 1) i8_update_kernel_wide(const __gr
 // Also accumulates, per row, the dropped diagonal pairs  sum_{s+t>=S} 2^-(12+7(s+t)) sum_k q_s q_t  (exact integer
 // sums, fp64 weights) into corr[slot][row] with slot = 512-column group: two warps -> two commutative adds.
 // ST > 0: the plane count is a compile-time constant, so the digit table q[ST][16] lives in registers and every loop over
-// planes / digit pairs is unrolled; ST = 0 keeps the run-time count (q in local memory: 512 B of stack per thread, the
-// reason this kernel took 24 ms per factorisation at N = 65536 -- 5x its HBM time).
+// planes / digit pairs is unrolled; ST = 0 keeps the run-time count (q in local memory: 512 B of stack per thread).
 template <int ST>
 __global__ void __launch_bounds__(256, 2) cut_digits_kernel_t(const double* __restrict__ mat, int64_t ld, const double* __restrict__ rs,
                                                            int64_t r0, int64_t nrows, int64_t c0, int64_t ncols,
@@ -1217,7 +751,7 @@ static EncodeTiledFn get_encode() {
     return fn;
 }
 
-// planes: S contiguous int8 matrices [rows][ldq]; box = 128 bytes (k) x 128 rows, 128-byte swizzle
+// planes: S int8 matrices [rows][ldq] (plane-major) or the chunk-major layout; box = 128 bytes (k) x BOXR rows, 128-byte swizzle
 Maps make_maps(int8_t* planes, int64_t plane_stride, int64_t rows, int64_t ldq, int S, int layout = 0, int l2promo = 3) {
     Maps m{};
     EncodeTiledFn enc = get_encode();
@@ -1234,142 +768,80 @@ Maps make_maps(int8_t* planes, int64_t plane_stride, int64_t rows, int64_t ldq, 
                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, promo,
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) throw GpError("cuTensorMapEncodeTiled (4-D) failed");
-        return m;   // the per-plane 2-D maps do not exist in this layout
+        return m;
     }
-    {
-        cuuint64_t dims[3] = {(cuuint64_t)ldq, (cuuint64_t)rows, (cuuint64_t)S};
-        cuuint64_t strides[2] = {(cuuint64_t)ldq, (cuuint64_t)plane_stride};
-        cuuint32_t box[3] = {(cuuint32_t)KC, (cuuint32_t)BOXR, 1u};
-        cuuint32_t estr[3] = {1u, 1u, 1u};
-        CUresult r = enc(&m.all, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, planes, dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, promo,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) throw GpError("cuTensorMapEncodeTiled (3-D) failed");
-    }
-    for (int s = 0; s < 8; ++s) {
-        const int sp = (s < S) ? s : 0;
-        cuuint64_t dims[2] = {(cuuint64_t)ldq, (cuuint64_t)rows};
-        cuuint64_t strides[1] = {(cuuint64_t)ldq};
-        cuuint32_t box[2] = {(cuuint32_t)KC, (cuuint32_t)BOXR};
-        cuuint32_t estr[2] = {1u, 1u};
-        CUresult r = enc(&m.plane[s], CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, planes + (int64_t)sp * plane_stride, dims, strides,
-                         box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                         promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) throw GpError("cuTensorMapEncodeTiled failed");
-    }
+    cuuint64_t dims[3] = {(cuuint64_t)ldq, (cuuint64_t)rows, (cuuint64_t)S};
+    cuuint64_t strides[2] = {(cuuint64_t)ldq, (cuuint64_t)plane_stride};
+    cuuint32_t box[3] = {(cuuint32_t)KC, (cuuint32_t)BOXR, 1u};
+    cuuint32_t estr[3] = {1u, 1u, 1u};
+    CUresult r = enc(&m.all, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, planes, dims, strides, box, estr,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, promo,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) throw GpError("cuTensorMapEncodeTiled (3-D) failed");
     return m;
 }
 
-template <int CM, int CN, bool PG>
+// cluster-tile geometry of a launch: ctm x ctn cluster tiles of (CM * ROWS) x (CN * CTN)
+struct ClusterGrid { int cs, ctm, ctn; int64_t rows, cols; };
+static ClusterGrid cluster_grid(const Args& a, int CM, int CN, int MW) {
+    ClusterGrid q;
+    q.cs = CM * CN;
+    q.rows = (int64_t)CM * 128 * MW;
+    q.cols = (int64_t)CN * CTN;
+    q.ctm = (int)(((int64_t)a.tiles_m * TM + q.rows - 1) / q.rows);
+    q.ctn = (int)(((int64_t)a.tiles_n * TN + q.cols - 1) / q.cols);
+    return q;
+}
+static bool cluster_above_diagonal(const Args& a, const ClusterGrid& q, int cid) {
+    const int ci = cid / q.ctn, cj = cid % q.ctn;
+    return a.skip_upper && a.row0 + (int64_t)ci * q.rows + q.rows - 1 < a.col0 + (int64_t)cj * q.cols;
+}
+
+template <int CM, int CN, bool PG, int MW>
 static void launch_cfg(b200gp_ctx* ctx, const Maps& maps, const Args& a) {
+    constexpr int SMEM = Geo<MW>::SMEM_BYTES;
     static bool attr = false;
     if (!attr) {
-        CUDA_CHECK(cudaFuncSetAttribute(i8_update_kernel<CM, CN, PG>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+        CUDA_CHECK(cudaFuncSetAttribute(i8_update_kernel<CM, CN, PG, MW>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
         attr = true;
     }
-    const int ctm = (a.tiles_m + CM - 1) / CM, ctn = (a.tiles_n + CN - 1) / CN;
-    const int64_t nclusters = (int64_t)ctm * ctn;
+    const ClusterGrid q = cluster_grid(a, CM, CN, MW);
+    const int64_t nclusters = (int64_t)q.ctm * q.ctn;
     if (nclusters <= 0 || a.K <= 0) return;
     cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)(nclusters * CM * CN));
+    cfg.gridDim = dim3((unsigned)((nclusters + (a.nseg > 1 ? (int64_t)(a.nseg - 1) * a.ntail : 0)) * q.cs));
     cfg.blockDim = dim3(THREADS);
-    cfg.dynamicSmemBytes = SMEM_BYTES;
+    cfg.dynamicSmemBytes = SMEM;
     cfg.stream = ctx->stream;
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = CM * CN;
+    at[0].val.clusterDim.x = q.cs;
     at[0].val.clusterDim.y = 1;
     at[0].val.clusterDim.z = 1;
     cfg.attrs = at;
     cfg.numAttrs = 1;
-    CUDA_CHECK(cudaLaunchKernelEx(&cfg, i8_update_kernel<CM, CN, PG>, maps, a));
+    CUDA_CHECK(cudaLaunchKernelEx(&cfg, i8_update_kernel<CM, CN, PG, MW>, maps, a));
     ctx->launches++;
     // int8 ops issued (mirrors the kernel's cluster-uniform decisions)
-    double pairs_tiles = 0.0;
-    for (int cj = 0; cj < ctn; ++cj)
-        for (int ci = 0; ci < ctm; ++ci) {
-            const int64_t rlo = a.row0 + (int64_t)ci * CM * TM, rhi = rlo + (int64_t)CM * TM - 1;
-            const int64_t clo = a.col0 + (int64_t)cj * CN * TN, chi = clo + (int64_t)CN * TN - 1;
-            if (a.skip_upper && rhi < clo) continue;
-            (void)chi;
-            pairs_tiles += (double)(CM * CN) * 0.5 * a.S * (a.S + 1);
-        }
-    ctx->prof.i8_ops += 2.0 * pairs_tiles * (double)TM * TN * (double)a.K;
+    int64_t active = 0;
+    for (int c = 0; c < nclusters; ++c) active += cluster_above_diagonal(a, q, c) ? 0 : 1;
+    ctx->prof.i8_ops += 2.0 * (double)active * 0.5 * a.S * (a.S + 1) * (double)q.rows * (double)q.cols * (double)a.K;
 }
 
-template <bool PG>
-static void launch_2sm(b200gp_ctx* ctx, const Maps& maps, const Args& a) {
-    static bool attr = false;
-    if (!attr) {
-        CUDA_CHECK(cudaFuncSetAttribute(i8_update_kernel_2sm<PG>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM2_BYTES));
-        attr = true;
-    }
-    const int ptm = (a.tiles_m + 1) / 2;
-    const int64_t npairs = (int64_t)ptm * a.tiles_n;
-    if (npairs <= 0 || a.K <= 0) return;
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)(2 * (npairs + (a.nseg > 1 ? (int64_t)(a.nseg - 1) * a.ntail : 0))));
-    cfg.blockDim = dim3(THREADS);
-    cfg.dynamicSmemBytes = SMEM2_BYTES;
-    cfg.stream = ctx->stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = 2;
-    at[0].val.clusterDim.y = 1;
-    at[0].val.clusterDim.z = 1;
-    cfg.attrs = at;
-    cfg.numAttrs = 1;
-    CUDA_CHECK(cudaLaunchKernelEx(&cfg, i8_update_kernel_2sm<PG>, maps, a));
-    ctx->launches++;
-    double pairs_tiles = 0.0;
-    for (int pi = 0; pi < ptm; ++pi)
-        for (int tj = 0; tj < a.tiles_n; ++tj) {
-            const int64_t rlo = a.row0 + (int64_t)pi * 2 * TM, clo = a.col0 + (int64_t)tj * TN;
-            if (a.skip_upper && rlo + 2 * TM - 1 < clo) continue;
-            pairs_tiles += 2.0 * 0.5 * a.S * (a.S + 1);
-        }
-    ctx->prof.i8_ops += 2.0 * pairs_tiles * (double)TM * TN * (double)a.K;
-}
-
-static void launch_wide(b200gp_ctx* ctx, const Maps& maps, const Args& a) {
-    static bool attr = false;
-    if (!attr) {
-        CUDA_CHECK(cudaFuncSetAttribute(i8_update_kernel_wide, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_W_BYTES));
-        attr = true;
-    }
-    const int ptm = (a.tiles_m + 1) / 2;
-    const int64_t nt = (int64_t)ptm * a.tiles_n;
-    if (nt <= 0 || a.K <= 0) return;
-    i8_update_kernel_wide<<<(unsigned)nt, THREADS_W, SMEM_W_BYTES, ctx->stream>>>(maps, a);
-    CUDA_CHECK(cudaGetLastError());
-    ctx->launches++;
-    double pairs_tiles = 0.0;
-    for (int pi = 0; pi < ptm; ++pi)
-        for (int tj = 0; tj < a.tiles_n; ++tj) {
-            const int64_t rlo = a.row0 + (int64_t)pi * 2 * TM, clo = a.col0 + (int64_t)tj * TN;
-            if (a.skip_upper && rlo + 2 * TM - 1 < clo) continue;
-            pairs_tiles += 2.0 * 0.5 * a.S * (a.S + 1);
-        }
-    ctx->prof.i8_ops += 2.0 * pairs_tiles * (double)TM * TN * (double)a.K;
-}
-
-// cluster shape code: 1 = wide 256 x 256 tile per CTA (two MMAs per B stage, no cluster);
-// 2 = CTA pair with tcgen05 cta_group::2 (256 x 256 tile per pair);
-// 11 = 1x1 (no multicast), 21 = 2x1, 12 = 1x2, 22 = 2x2, 41 = 4x1, 42 = 4x2 (cta_group::1 + TMA multicast)
+// cluster shape code: 1 = wide 256 x 128 tile per CTA (both m64 blocks of a warpgroup share every B stage; no pairing, no
+// cluster); 2 = 2 x 1 cluster (B slices multicast to the CTA below, 256 x 128 per cluster) with tail split-K (default);
+// 11 = 1x1 (no multicast), 21 = 2x1, 12 = 1x2, 22 = 2x2, 41 = 4x1, 42 = 4x2 (CTA tiles of 128 x 128, TMA multicast)
 static void launch_update_one(b200gp_ctx* ctx, const Maps& maps, const Args& a) {
-    if (a.layout == 1 && (ctx->oz_cluster == 1 || ctx->oz_cluster == 2))
-        throw GpError("ozaki_layout=1 (chunk-major digit planes) is not implemented for the wide / 2-SM kernels");
+    if (ctx->oz_cluster == 1) { launch_cfg<1, 1, false, 2>(ctx, maps, a); return; }
     switch ((int)ctx->oz_cluster) {
-        case 1: launch_wide(ctx, maps, a); break;
-        case 2: if (ctx->oz_pairing) launch_2sm<true>(ctx, maps, a); else launch_2sm<false>(ctx, maps, a); break;
 #define OZ_CFG(CMv, CNv) \
-    do { if (ctx->oz_pairing) launch_cfg<CMv, CNv, true>(ctx, maps, a); else launch_cfg<CMv, CNv, false>(ctx, maps, a); } while (0)
+    do { if (ctx->oz_pairing) launch_cfg<CMv, CNv, true, 1>(ctx, maps, a); else launch_cfg<CMv, CNv, false, 1>(ctx, maps, a); } while (0)
         case 11: OZ_CFG(1, 1); break;
-        case 21: OZ_CFG(2, 1); break;
         case 12: OZ_CFG(1, 2); break;
+        case 22: OZ_CFG(2, 2); break;
         case 41: OZ_CFG(4, 1); break;
         case 42: OZ_CFG(4, 2); break;
-        default: OZ_CFG(2, 2); break;
+        default: OZ_CFG(2, 1); break;   // 2 and 21
 #undef OZ_CFG
     }
 }
@@ -1384,59 +856,55 @@ int max_exact_k(int S) {
     return (int)((k / KC) * KC);
 }
 
-// tail tile `ti` (pair index split_from + ti): C[tile] += sum_s scratch[s][ti] in the fixed order s = 0, 1, ... (deterministic)
+// tail cluster tile `ti` (cluster index split_from + ti): C[tile] += sum_s scratch[s][ti] in the fixed order s = 0, 1, ...
+// (deterministic)
 __global__ void __launch_bounds__(256) splitk_fixup_kernel(double* __restrict__ C, int64_t ldc, int64_t row0, int64_t col0,
-                                                           int tiles_n, int split_from, int ntail, int nextra,
-                                                           const double* __restrict__ scr, int64_t n_rows) {
+                                                           int ctn, int64_t trows, int64_t tcols, int split_from, int ntail,
+                                                           int nextra, const double* __restrict__ scr, int64_t n_rows) {
     const int ti = blockIdx.y;
-    const int pair = split_from + ti, pi = pair / tiles_n, tj = pair % tiles_n;
-    const int64_t prow0 = row0 + (int64_t)pi * 2 * TM, gcol0 = col0 + (int64_t)tj * TN;
-    const int idx = blockIdx.x * blockDim.x + threadIdx.x;          // 2 columns per thread: 256 rows x 128 column pairs
-    const int r = idx >> 7, c = (idx & 127) * 2;
-    if (r >= 2 * TM || prow0 + r >= n_rows || gcol0 + c >= n_rows) return;
+    const int cid = split_from + ti, ci = cid / ctn, cj = cid % ctn;
+    const int64_t prow0 = row0 + (int64_t)ci * trows, gcol0 = col0 + (int64_t)cj * tcols;
+    const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;   // 2 columns per thread
+    const int64_t r = idx / (tcols / 2), c = (idx % (tcols / 2)) * 2;
+    if (r >= trows || prow0 + r >= n_rows || gcol0 + c >= n_rows) return;
     double2* cp = reinterpret_cast<double2*>(C + (prow0 + r) * ldc + gcol0 + c);
     double2 v = *cp;
     for (int sg = 0; sg < nextra; ++sg) {
-        const double2 w = *reinterpret_cast<const double2*>(scr + ((int64_t)sg * ntail + ti) * (2 * TM * TN) + r * TN + c);
+        const double2 w = *reinterpret_cast<const double2*>(scr + ((int64_t)sg * ntail + ti) * (trows * tcols) + r * tcols + c);
         v.x += w.x; v.y += w.y;
     }
     *cp = v;
 }
 
-// Split-K of the CTA-pair kernel's LAST, partially filled wave (option "ozaki_splitk" = E > 0: on, E = cost of a tile's
-// fixed part -- four epilogue passes, pipeline fill -- in K columns; 0 = off).  A block-column launch has T active
-// 256 x 256 tiles of EQUAL duration for `slots` SM pairs: floor(T / slots) full waves and a last wave of r = T mod slots
-// tiles that leaves slots - r SM pairs idle for a whole tile time; the last block columns have the longest tiles and the
-// fewest of them (T = 10 at K = 64512 for the last column of N = 65536: 13 % of the chip busy).  The r tail tiles -- the
-// last pair indices of the launch, scheduled last -- are cut into s = floor(slots / r) K segments that run as s r <= slots
-// short tiles of the SAME launch: segment 0 updates C, segment sg >= 1 accumulates into its own zero-filled fp64 scratch
-// tile, added to C afterwards in a fixed order.  Every segment's integer sums are exact, so the only change is the order
-// of s fp64 additions per element of a tail tile.  Scratch: r (s - 1) x 512 KB <= 37 MB.
+// Split-K of the default (code 2) launch's LAST, partially filled wave (option "ozaki_splitk" = E > 0: on, E = cost of a
+// tile's fixed part -- epilogue passes, pipeline fill -- in K columns; 0 = off).  A block-column launch has T active cluster
+// tiles of EQUAL duration for `slots` SM pairs: floor(T / slots) full waves and a last wave of r = T mod slots tiles that
+// leaves slots - r SM pairs idle for a whole tile time; the last block columns have the longest tiles and the fewest of
+// them.  The r tail tiles -- the last cluster indices of the launch, scheduled last -- are cut into s = floor(slots / r) K
+// segments that run as s r <= slots short tiles of the SAME launch: segment 0 updates C, segment sg >= 1 accumulates into its
+// own zero-filled fp64 scratch tile, added to C afterwards in a fixed order.  Every segment's integer sums are exact, so the
+// only change is the order of s fp64 additions per element of a tail tile.
 struct SplitPlan { int nseg = 1, kseg = 0, split_from = 0, ntail = 0; };
-static SplitPlan choose_splitk(b200gp_ctx* ctx, const Args& a) {
+static SplitPlan choose_splitk(b200gp_ctx* ctx, const Args& a, const ClusterGrid& q) {
     SplitPlan p;
     p.kseg = a.K;
     const int64_t E = ctx->oz_splitk;
     if (ctx->oz_cluster != 2 || a.no_split || a.K < 2 * KC) return p;
-    const int ptm = (a.tiles_m + 1) / 2, npairs = ptm * a.tiles_n;
+    const int nclus = q.ctm * q.ctn;
     auto seg_len = [&](int s) { return (int)((((int64_t)a.K + s - 1) / s + KC - 1) / KC) * KC; };
     if (ctx->oz_splitk_force > 1) {   // tests: every tile, this many segments whatever the cost model says
         int s = (int)ctx->oz_splitk_force;
         if (s > a.K / KC) s = a.K / KC;
         p.kseg = seg_len(s);
         p.nseg = (a.K + p.kseg - 1) / p.kseg;
-        p.split_from = 0; p.ntail = npairs;
+        p.split_from = 0; p.ntail = nclus;
         return p;
     }
     if (E <= 0) return p;
-    const int slots = ctx->num_sms / 2 > 0 ? ctx->num_sms / 2 : 1;
-    // active tiles in launch order (pair index = pi * tiles_n + tj); the tail starts at the (full waves * slots)-th one
+    const int slots = ctx->num_sms / q.cs > 0 ? ctx->num_sms / q.cs : 1;
+    // active tiles in launch order; the tail starts at the (full waves * slots)-th one
     int64_t active = 0;
-    for (int pr = 0; pr < npairs; ++pr) {
-        const int pi = pr / a.tiles_n, tj = pr % a.tiles_n;
-        if (a.skip_upper && a.row0 + (int64_t)pi * 2 * TM + 2 * TM - 1 < a.col0 + (int64_t)tj * TN) continue;
-        ++active;
-    }
+    for (int c = 0; c < nclus; ++c) active += cluster_above_diagonal(a, q, c) ? 0 : 1;
     const int64_t r = active % slots, full = active - r;
     if (r == 0) return p;
     int s = (int)(slots / r);
@@ -1447,22 +915,22 @@ static SplitPlan choose_splitk(b200gp_ctx* ctx, const Args& a) {
     // worth it?  tail wave (K + E) against (kseg + E) + scratch traffic (zero-fill, fix-up) ~ 0.02 K-columns per tile-segment
     if ((double)kseg + (double)E > 0.9 * ((double)a.K + (double)E) || nseg < 2) return p;
     int64_t seen = 0;
-    int split_from = npairs;
-    for (int pr = 0; pr < npairs; ++pr) {
-        const int pi = pr / a.tiles_n, tj = pr % a.tiles_n;
-        if (a.skip_upper && a.row0 + (int64_t)pi * 2 * TM + 2 * TM - 1 < a.col0 + (int64_t)tj * TN) continue;
-        if (seen == full) { split_from = pr; break; }
+    int split_from = nclus;
+    for (int c = 0; c < nclus; ++c) {
+        if (cluster_above_diagonal(a, q, c)) continue;
+        if (seen == full) { split_from = c; break; }
         ++seen;
     }
-    if (split_from >= npairs) return p;
-    p.nseg = nseg; p.kseg = kseg; p.split_from = split_from; p.ntail = npairs - split_from;
+    if (split_from >= nclus) return p;
+    p.nseg = nseg; p.kseg = kseg; p.split_from = split_from; p.ntail = nclus - split_from;
     return p;
 }
 
 static void launch_update_splitk(b200gp_ctx* ctx, const Maps& maps, const Args& a) {
-    const SplitPlan p = choose_splitk(ctx, a);
+    const ClusterGrid q = cluster_grid(a, 2, 1, 1);   // the code-2 launch shape
+    const SplitPlan p = choose_splitk(ctx, a, q);
     if (p.nseg <= 1) { launch_update_one(ctx, maps, a); return; }
-    const size_t tile_doubles = (size_t)2 * TM * TN;
+    const size_t tile_doubles = (size_t)(q.rows * q.cols);
     const size_t need = (size_t)(p.nseg - 1) * p.ntail * tile_doubles * 8;
     size_t scr_bytes = (size_t)64 << 20;    // size classes (powers of two) so that the context's buffer cache hits
     while (scr_bytes < need) scr_bytes <<= 1;
@@ -1472,9 +940,9 @@ static void launch_update_splitk(b200gp_ctx* ctx, const Maps& maps, const Args& 
     b.nseg = p.nseg; b.kseg = p.kseg; b.split_from = p.split_from; b.ntail = p.ntail;
     b.Cseg = scr.f64();
     launch_update_one(ctx, maps, b);
-    dim3 grid((unsigned)((2 * TM * (TN / 2) + 255) / 256), (unsigned)p.ntail);
-    splitk_fixup_kernel<<<grid, 256, 0, ctx->stream>>>(a.C, a.ldc, a.row0, a.col0, a.tiles_n, p.split_from, p.ntail, p.nseg - 1,
-                                                      scr.f64(), a.n_rows);
+    dim3 grid((unsigned)((tile_doubles / 2 + 255) / 256), (unsigned)p.ntail);
+    splitk_fixup_kernel<<<grid, 256, 0, ctx->stream>>>(a.C, a.ldc, a.row0, a.col0, q.ctn, q.rows, q.cols, p.split_from, p.ntail,
+                                                      p.nseg - 1, scr.f64(), a.n_rows);
     CUDA_CHECK(cudaGetLastError());
     ctx->launches++;
 }
@@ -1493,84 +961,29 @@ void launch_update(b200gp_ctx* ctx, const Maps& maps, const Args& a) {
     }
 }
 
-// ---- int8 tensor peak: MMAs back to back from resident smem operands --------------------------------------
-__global__ void __launch_bounds__(128, 1) i8_peak_kernel(int iters, int* sink) {
+// ---- int8 tensor peak: wgmma back to back from resident shared-memory operands (both warpgroups of every SM) ----------
+constexpr int PEAK_SMEM = 2 * 64 * KC + B_BYTES + 1024;
+__global__ void __launch_bounds__(256, 1) i8_peak_kernel(int iters, int* sink) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t* bar = reinterpret_cast<uint64_t*>(smem + STAGE_BYTES);
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bar + 1);
-    volatile int* abort_flag = reinterpret_cast<volatile int*>(tmem_ptr + 1);
-    for (int i = threadIdx.x; i < STAGE_BYTES / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(smem)[i] = 0x01010101u;
-    if (threadIdx.x == 0) {
-        mbar_init(bar, 1);
-        *abort_flag = 0;
-        asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-    }
-    asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");   // generic-proxy smem writes -> async proxy (UMMA)
-    if ((threadIdx.x >> 5) == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;\n" ::"r"(smem_u32(tmem_ptr)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-    }
-    tc_fence_before();
+    for (int i = threadIdx.x; i < (2 * 64 * KC + B_BYTES) / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(smem)[i] = 0x01010101u;
+    asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");   // generic-proxy smem writes -> async proxy (wgmma)
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
-    if (threadIdx.x == 32) {
-        const uint32_t a_addr = smem_u32(smem), b_addr = a_addr + A_BYTES;
-        for (int it = 0; it < iters; ++it) {
+    const int wg = threadIdx.x >> 7;
+    const uint32_t a_addr = smem_u32(smem) + (uint32_t)(wg * 64 * KC), b_addr = smem_u32(smem) + 2 * 64 * KC;
+    uint32_t d[64];
 #pragma unroll
-            for (int kk = 0; kk < 4; ++kk)
-                umma_i8(tmem_base + (uint32_t)((it & 1) * TN), make_desc(a_addr + kk * 32), make_desc(b_addr + kk * 32), 1u);
-        }
-        tc_commit(bar);
-        if (!mbar_wait(bar, 0, abort_flag)) atomicExch(sink, 1);
+    for (int i = 0; i < 64; ++i) d[i] = 0;
+    wg_fence();
+    for (int it = 0; it < iters; ++it) {
+        uint32_t acc = 1;
+        mma_stage(d, a_addr, b_addr, acc);
+        wg_commit();
+        wg_wait1();
     }
-    tc_fence_before();
-    __syncthreads();
-    if ((threadIdx.x >> 5) == 1)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;\n" ::"r"(tmem_base) : "memory");
-}
-
-// same with cta_group::2 (CTA pair, M = 256): does the 2-SM MMA itself run at full rate?
-__global__ void __launch_bounds__(128, 1) i8_peak_kernel_2sm(int iters, int* sink) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t* bar = reinterpret_cast<uint64_t*>(smem + STAGE2_BYTES);
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bar + 1);
-    volatile int* abort_flag = reinterpret_cast<volatile int*>(tmem_ptr + 1);
-    int crank;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;\n" : "=r"(crank));
-    for (int i = threadIdx.x; i < STAGE2_BYTES / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(smem)[i] = 0x01010101u;
-    if (threadIdx.x == 0) {
-        mbar_init(bar, 1);
-        *abort_flag = 0;
-        asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-    }
-    asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
-    if ((threadIdx.x >> 5) == 1) {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], 512;\n" ::"r"(smem_u32(tmem_ptr)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;\n" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
-    if (crank == 0 && threadIdx.x == 32) {
-        const uint32_t a_addr = smem_u32(smem), b_addr = a_addr + A_BYTES;
-        for (int it = 0; it < iters; ++it) {
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk)
-                umma_i8_2sm(tmem_base + (uint32_t)((it & 1) * TN), make_desc(a_addr + kk * 32), make_desc(b_addr + kk * 32), 1u);
-        }
-        tc_commit_2sm(bar, 0x1);
-        if (!mbar_wait(bar, 0, abort_flag)) atomicExch(sink, 1);
-    }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    if ((threadIdx.x >> 5) == 1)
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, 512;\n" ::"r"(tmem_base) : "memory");
+    wg_wait0();
+    // every product is 1 x 1 summed over K = 128 per stage: the result is known, a wrong one marks the measurement invalid
+    if (d[0] != (uint32_t)iters * (uint32_t)KC) atomicExch(sink, 1);
 }
 
 }  // namespace oz
@@ -1938,55 +1351,26 @@ extern "C" int b200gp_i8_update_bench(b200gp_ctx* ctx, int64_t rows, int64_t col
 
 extern "C" int b200gp_measure_i8_peak(b200gp_ctx* ctx, double* tops) {
     API_BEGIN(ctx)
-    const int smem_bytes = oz::STAGE_BYTES + 1024 + 64;
-    CUDA_CHECK(cudaFuncSetAttribute(oz::i8_peak_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+    CUDA_CHECK(cudaFuncSetAttribute(oz::i8_peak_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, oz::PEAK_SMEM));
     int* sink = (int*)_ctx->alloc(sizeof(int));
     CUDA_CHECK(cudaMemsetAsync(sink, 0, sizeof(int), _ctx->stream));
     const int iters = (int)((_ctx->peak_iters < 200000) ? _ctx->peak_iters * 4 : 800000);
     float ms = 0;
     for (int rep = 0; rep < 2; ++rep) {
         cudaEventRecord(_ctx->ev0, _ctx->stream);
-        oz::i8_peak_kernel<<<_ctx->num_sms, 128, smem_bytes, _ctx->stream>>>(iters, sink);
+        oz::i8_peak_kernel<<<_ctx->num_sms, 256, oz::PEAK_SMEM, _ctx->stream>>>(iters, sink);
         cudaEventRecord(_ctx->ev1, _ctx->stream);
         CUDA_CHECK(cudaEventSynchronize(_ctx->ev1));
         cudaEventElapsedTime(&ms, _ctx->ev0, _ctx->ev1);
     }
     CUDA_CHECK(cudaGetLastError());
     _ctx->launches += 2;
-    *tops = (double)_ctx->num_sms * (double)iters * 4.0 * 2.0 * oz::TM * oz::TN * 32.0 / (ms * 1e-3) / 1e12;
+    int bad = 0;
+    CUDA_CHECK(cudaMemcpy(&bad, sink, sizeof(int), cudaMemcpyDeviceToHost));
     _ctx->release(sink, sizeof(int));
-    API_END
-}
-
-extern "C" int b200gp_measure_i8_peak_2sm(b200gp_ctx* ctx, double* tops) {
-    API_BEGIN(ctx)
-    const int smem_bytes = oz::STAGE2_BYTES + 1024 + 64;
-    CUDA_CHECK(cudaFuncSetAttribute(oz::i8_peak_kernel_2sm, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-    int* sink = (int*)_ctx->alloc(sizeof(int));
-    CUDA_CHECK(cudaMemsetAsync(sink, 0, sizeof(int), _ctx->stream));
-    const int iters = (int)((_ctx->peak_iters < 200000) ? _ctx->peak_iters * 4 : 800000);
-    const int npairs = _ctx->num_sms / 2;
-    float ms = 0;
-    for (int rep = 0; rep < 2; ++rep) {
-        cudaLaunchConfig_t cfg{};
-        cfg.gridDim = dim3((unsigned)(npairs * 2));
-        cfg.blockDim = dim3(128);
-        cfg.dynamicSmemBytes = smem_bytes;
-        cfg.stream = _ctx->stream;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeClusterDimension;
-        at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-        cfg.attrs = at; cfg.numAttrs = 1;
-        cudaEventRecord(_ctx->ev0, _ctx->stream);
-        CUDA_CHECK(cudaLaunchKernelEx(&cfg, oz::i8_peak_kernel_2sm, iters, sink));
-        cudaEventRecord(_ctx->ev1, _ctx->stream);
-        CUDA_CHECK(cudaEventSynchronize(_ctx->ev1));
-        cudaEventElapsedTime(&ms, _ctx->ev0, _ctx->ev1);
-    }
-    _ctx->launches += 2;
-    // per pair per instruction: 256 x 256 x 32 MAC
-    *tops = (double)npairs * (double)iters * 4.0 * 2.0 * 256.0 * 256.0 * 32.0 / (ms * 1e-3) / 1e12;
-    _ctx->release(sink, sizeof(int));
+    if (bad) throw GpError("i8 peak: wrong accumulator value");
+    // per SM and iteration: 2 warpgroups x 4 instructions x 64 x 128 x 32 MAC
+    *tops = (double)_ctx->num_sms * (double)iters * 2.0 * 4.0 * 2.0 * 64.0 * oz::CTN * 32.0 / (ms * 1e-3) / 1e12;
     API_END
 }
 

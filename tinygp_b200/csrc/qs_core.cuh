@@ -356,8 +356,7 @@ __host__ __device__ __forceinline__ void strow(double* p, int64_t k, const doubl
 // ---------------------------------------------------------------------------------------------
 // 32-byte per-thread vector accesses.  One thread walks `chunk` consecutive points, so neighbouring threads are
 // chunk*8 bytes apart and nothing coalesces across the warp; with scalar loads every thread keeps ~5 cache
-// lines "hot" and 1024 resident threads thrash L1 (ncu, round 1: all four scan kernels cost ~0.65 ms regardless
-// of their flop count).  Loading/storing 4 points (one full 32-byte sector) per access makes every sector move
+// lines "hot" and 1024 resident threads thrash L1.  Loading/storing 4 points (one full 32-byte sector) per access makes every sector move
 // exactly once.
 // ---------------------------------------------------------------------------------------------
 __host__ __device__ __forceinline__ void ld4(const double* __restrict__ p, int64_t kb, int64_t k1, double (&v)[4]) {

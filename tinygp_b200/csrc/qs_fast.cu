@@ -5,8 +5,8 @@
 #include "qs_fast.cuh"
 
 // MINB: minimum resident blocks per SM asked of the compiler (register cap 65536 / (128 * MINB)): the fold / replay bodies
-// want ~154 / ~222 registers, i.e. 3 / 2 blocks = 12 / 8 warps per SM, and ncu shows the fp64 pipe only 57 % / 42 % busy at
-// that occupancy; MINB = 4 / 3 costs ~100 bytes of spills per thread and buys 16 / 12 warps.
+// want ~154 / ~222 registers, i.e. 3 / 2 blocks = 12 / 8 warps per SM; MINB = 4 / 3 trades ~100 bytes of spills per thread
+// for 16 / 12 warps.
 template <int L, int MINB>
 __global__ void __launch_bounds__(QS_THREADS, MINB) qsf_chunk_kernel(const __grid_constant__ QsModel m, const __grid_constant__ QsFastConst fc,
                                                                const double* __restrict__ t, const double* __restrict__ diag,
@@ -39,8 +39,8 @@ __global__ void __launch_bounds__(256) qsf_finish_kernel(const double* quad, con
 
 // factor (c, w, sum log c, info) and -- with x_fuse -- sum of squares of the forward substitution L^-1 x, all on the stream
 template <int L>
-static void qsf_run(b200gp_qs* s, const double* t, const double* diag, int* info_dev, double* logdet_dev, const double* x_fuse,
-                    double* sumsq_dev) {
+void qsf_run(b200gp_qs* s, const double* t, const double* diag, int* info_dev, double* logdet_dev, const double* x_fuse,
+             double* sumsq_dev) {
     constexpr int J = lay_J(L);
     b200gp_ctx* ctx = s->ctx;
     const int64_t n = s->n, nch = (n + s->model.chunk - 1) / s->model.chunk;
@@ -75,7 +75,7 @@ static void qsf_run(b200gp_qs* s, const double* t, const double* diag, int* info
 }
 
 template <int L>
-static void qsf_solvesq_run(b200gp_qs* s, const double* x, double* sumsq_dev) {
+void qsf_solvesq_run(b200gp_qs* s, const double* x, double* sumsq_dev) {
     constexpr int J = lay_J(L);
     b200gp_ctx* ctx = s->ctx;
     const int64_t n = s->n, nch = (n + s->model.chunk - 1) / s->model.chunk;
@@ -91,6 +91,20 @@ static void qsf_solvesq_run(b200gp_qs* s, const double* x, double* sumsq_dev) {
     sum_partials(ctx, part.f64(), nch, sumsq_dev);
     CUDA_CHECK(cudaGetLastError());
 }
+
+#ifdef QSF_PART_LAYOUTS
+// an instantiation unit (qs_fast_p*.cu): the kernels of a few layouts, so that the layouts compile in parallel
+#define X(code)                                                                                                           \
+    template void qsf_run<code>(b200gp_qs*, const double*, const double*, int*, double*, const double*, double*);         \
+    template void qsf_solvesq_run<code>(b200gp_qs*, const double*, double*);
+QSF_PART_LAYOUTS(X)
+#undef X
+#else
+#define X(code)                                                                                                           \
+    extern template void qsf_run<code>(b200gp_qs*, const double*, const double*, int*, double*, const double*, double*);  \
+    extern template void qsf_solvesq_run<code>(b200gp_qs*, const double*, double*);
+QSF_LAYOUTS(X)
+#undef X
 
 // |L^-1 x|^2 for an existing factor; false if the layout is not compiled in
 bool qsf_solve_sumsq(b200gp_qs* s, const double* x_dev, double* sumsq_dev) {
@@ -123,3 +137,4 @@ bool qsf_factor(b200gp_qs* s, const double* t, const double* diag, int* info_dev
         default: return false;
     }
 }
+#endif

@@ -1,4 +1,4 @@
-// Structured fast path of the quasiseparable log-probability / factorisation (round 2).
+// Structured fast path of the quasiseparable log-probability / factorisation.
 //
 // Same mathematics as qs_core.cuh (reference: src/tinygp/solvers/quasisep/ops.py:352-399, :463-486 and the state-space
 // models of src/tinygp/kernels/quasisep.py:404-673), specialised at COMPILE TIME on the block layout of the model:
@@ -6,7 +6,7 @@
 // of size 1 (Exp), 2 (Matern32, SHO, Celerite, Cosine) or 3 (Matern52) per component.  A layout is encoded as base-4
 // digits (first block = least significant digit), e.g. SHO + Matern32 -> {2, 2} -> 2 + 2*4 = 10.
 //
-// What the specialisation buys over the generic J x J code of qs_core.cuh (ALU-bound: ncu round 1/2):
+// What the specialisation buys over the generic J x J code of qs_core.cuh (ALU-bound):
 //   * the generators land in registers with compile-time offsets (the generic qs_gen assembles them through a
 //     runtime-indexed scratch array = local memory, 176 bytes of stack per thread);
 //   * every product with `a` skips the structurally zero blocks (J = 4, {2,2}: 32 instead of 64 FMA per product);

@@ -99,7 +99,7 @@ static __global__ void sum_partials_kernel(const double* part, int64_t n, double
 static inline unsigned nblk(int64_t n, int t) { return (unsigned)((n + t - 1) / t); }
 
 // fixed-shape (deterministic) sum of n per-chunk partials: one block per slab of 8192 values, then one block over the
-// slab sums -- the single-block version took 18 us for the 156250 chunks of an N = 1e7 series (ncu launch list, round 2)
+// slab sums (a single block over all chunks of a long series is a serial tail)
 static __global__ void sum_slabs_kernel(const double* part, int64_t n, double* slab_sums) {
     __shared__ double sh[256];
     const int64_t lo = (int64_t)blockIdx.x * 8192, hi = (lo + 8192 < n) ? lo + 8192 : n;

@@ -136,7 +136,7 @@ static void run_ew(b200gp_ctx* ctx, const Args& a, int64_t total) {
     ctx->launches++;
 #else
     int64_t blocks = (total + 255) / 256;
-    if (blocks > 148 * 32) blocks = 148 * 32;
+    if (blocks > (int64_t)ctx->num_sms * 32) blocks = (int64_t)ctx->num_sms * 32;
     qsm_ew_kernel<Args, Fn><<<(unsigned)blocks, 256, 0, ctx->stream>>>(a, total);
     CUDA_CHECK(cudaGetLastError());
     ctx->launches++;

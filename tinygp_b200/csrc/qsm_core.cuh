@@ -1,4 +1,4 @@
-// Quasiseparable-matrix algebra on generator ARRAYS (row f2 / a30 of SURVEY section 8): the per-chunk bodies of the
+// Quasiseparable-matrix algebra on generator ARRAYS: the per-chunk bodies of the
 // scans behind src/tinygp/solvers/quasisep/core.py and ops.py for matrices whose generators are arbitrary per-point
 // arrays (d (n), p, q (n x m), a (n x m x m)) of any order m -- the conditioned covariance of solver.py:124-129 has
 // order 4J, its `a` is a dense 16 x 16 block per point at J = 4.

@@ -1,4 +1,4 @@
-// QuasisepSolver path for sm_100a: the celerite recursions as chunked three-phase scans.
+// QuasisepSolver path for sm_90a: the celerite recursions as chunked three-phase scans.
 //
 // Reference behaviour being replaced: src/tinygp/solvers/quasisep/solver.py:35-139,
 // src/tinygp/solvers/quasisep/ops.py:308-365,463-512 (sequential scans; the parallel forms :319-399,
@@ -19,6 +19,9 @@
 // HBM traffic per point: read t, diag (and y) ; write c, w  -- 8(3 + 1 + J) bytes for log_probability.
 #include "qs_generic.cuh"
 
+QS_FOR_J(extern template, 4)      // quasisep_j4.cu
+QS_FOR_J(extern template, 5)      // quasisep_j5.cu
+QS_FOR_J(extern template, 6)      // quasisep_j6.cu
 QS_FOR_J(extern template, 7)      // quasisep_j7.cu
 QS_FOR_J(extern template, 8)      // quasisep_j8.cu
 

@@ -1,0 +1,5 @@
+// The generic quasiseparable scans for state dimension J = 6 (see qs_generic.cuh): a translation unit of its own so that
+// it compiles in parallel with quasisep.cu.
+#include "qs_generic.cuh"
+
+QS_FOR_J(template, 6)

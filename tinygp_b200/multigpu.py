@@ -3,7 +3,7 @@
 The int8 tensor-core trailing update of block column J is split by ROWS over the ranks; one
 ``all_gather_into_tensor`` per block column (NCCL over NVLink, rows x nb x 8 bytes) gives every rank the whole
 updated column, and every rank then factors the panel and cuts its digits redundantly (cheap, deterministic),
-so there is no panel broadcast.  See ``include/b200gp.h`` (b200gp_mg_*) and DESIGN.md section 5.
+so there is no panel broadcast.  See ``include/b200gp.h`` (b200gp_mg_*).
 """
 
 from __future__ import annotations

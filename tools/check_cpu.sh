@@ -1,6 +1,6 @@
 #!/usr/bin/env bash
 # Everything that can be checked without a GPU, in the order the round-end driver does it:
-#   1. build(): nvcc cross-compiles libb200gp.so for sm_100a, gcc builds the C oracle (+ oracle/_ref when the reference is here)
+#   1. build(): nvcc cross-compiles libb200gp.so for sm_90a, gcc builds the C oracle (+ oracle/_ref when the reference is here)
 #   2. the CPU test suite (oracle vs reference goldens, host layer over the mock C-ABI, device source compiled for the host,
 #      C-ABI symbols, gloo world_size 2)
 #   3. the GPU test files' host-side Python over the mock C-ABI (catches host-level errors in `-m gpu` tests before a GPU call;
