@@ -99,6 +99,8 @@ typedef struct {
     double qs_bytes;    /* algorithmic bytes moved by them                */
     int64_t qs_launches;
     double i8_ops;      /* int8 tensor ops (2 x MAC) issued by the fixed-point update launches (time: syrk_ms) */
+    double trtri_ms;    /* b200gp_dense_log_probability_grad: in-place triangular inverse L^-1 */
+    double contract_ms; /* b200gp_dense_log_probability_grad: mirror + W tiles + derivative epilogue + reductions */
 } b200gp_profile;
 int b200gp_get_profile(b200gp_ctx* ctx, b200gp_profile* out, int reset);
 
@@ -180,6 +182,24 @@ int b200gp_dense_log_probability(b200gp_ctx* ctx, const double* prog, int n_inst
 int b200gp_dense_log_probability_dev(b200gp_ctx* ctx, const double* prog, int n_instr,
                                      const double* X_dev, int64_t n, int ndim,
                                      const double* diag_dev, const double* resid_dev, double* logp);
+/* log_probability (gp.py:313-320, as b200gp_dense_log_probability) and its gradient, for a fresh factor that this call
+ * builds and frees.  With r = resid, alpha = K^-1 r and W = K^-1:
+ *   d logp / d theta = 1/2 sum_ij (alpha_i alpha_j - W_ij) dK_ij / d theta,   d logp / d diag_i = 1/2 (alpha_i^2 - W_ii).
+ * Outputs (host):
+ *   dprog   n_instr x 4, the program's shape: for each instruction row, column 2 = d logp / d p0 (leaf scale or CONST
+ *           value) and column 3 = d logp / d p1 (ExpSineSquared gamma, RationalQuadratic alpha); 0 everywhere else,
+ *           metric-definition rows included;
+ *   dmetric B200GP_PROG_MAX_METRICS x B200GP_METRIC_MAX_DIM: entry (m, r) = d logp / d lambda at lambda = 1 when row r
+ *           of metric m + 1 is scaled by lambda (0 for rows / metrics the program does not have);
+ *   ddiag   n;  alpha  n (= d logp / d mean = -d logp / d y).
+ * At most 16 differentiable scalars per program (one per leaf scale, CONST, gamma / alpha, metric row); programs with
+ * more, or with the closed forms of quasiseparable kernels (B200GP_OP_EXPCOS / EXPSIN), are refused.  L^-1 is formed
+ * in place and W is never stored: peak memory is that of b200gp_dense_log_probability plus O(n) per-row buffers.
+ * Deterministic: no floating-point atomics.  Non positive-definite input does not fail: logp = -inf and every gradient
+ * output is NaN. */
+int b200gp_dense_log_probability_grad(b200gp_ctx* ctx, const double* prog, int n_instr, const double* X, int64_t n,
+                                      int ndim, const double* diag, const double* resid, double* logp, double* dprog,
+                                      double* dmetric, double* ddiag, double* alpha);
 /* batched hyper-parameter grid (BASELINE config 5): nbatch programs of equal length over one X;
  * diag (n) and resid (n) shared.  logp[nbatch]. */
 int b200gp_dense_log_probability_batched(b200gp_ctx* ctx, const double* progs, int n_instr,

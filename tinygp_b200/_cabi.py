@@ -33,7 +33,7 @@ class Profile(ctypes.Structure):
         ("syrk_ms", c_double), ("syrk_flop", c_double), ("syrk_launches", c_int64),
         ("panel_ms", c_double), ("build_ms", c_double), ("build_bytes", c_double),
         ("solve_ms", c_double), ("qs_ms", c_double), ("qs_bytes", c_double),
-        ("qs_launches", c_int64), ("i8_ops", c_double),
+        ("qs_launches", c_int64), ("i8_ops", c_double), ("trtri_ms", c_double), ("contract_ms", c_double),
     ]
 
 
@@ -70,6 +70,7 @@ SIGNATURES = {
     "b200gp_dense_log_probability": (c_int, [_V, _D, _I, _D, _L, _I, _D, _D, c_double_p]),
     "b200gp_dense_log_probability_dev": (c_int, [_V, _D, _I, _D, _L, _I, _D, _D, c_double_p]),
     "b200gp_dense_log_probability_batched": (c_int, [_V, _D, _I, _L, _D, _L, _I, _D, _D, _D]),
+    "b200gp_dense_log_probability_grad": (c_int, [_V, _D, _I, _D, _L, _I, _D, _D, c_double_p, _D, _D, _D, _D]),
     "b200gp_mg_create": (c_int, [_V, _D, _I, _D, _L, _I, _D, _D, _I, _I, POINTER(c_void_p)]),
     "b200gp_mg_free": (c_int, [_V]),
     "b200gp_mg_use_colbuf": (c_int, [_V, _D, _L]),

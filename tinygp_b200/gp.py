@@ -6,13 +6,14 @@ the six ``Solver`` methods exactly where the reference calls them (gp.py:120,124
 
 from __future__ import annotations
 
-__all__ = ["GaussianProcess", "ConditionResult"]
+__all__ = ["GaussianProcess", "ConditionResult", "LogProbabilityGrad"]
 
+import copy
 from typing import Any, NamedTuple
 
 import numpy as np
 
-from tinygp_b200 import kernels, means
+from tinygp_b200 import kernels, means, transforms
 from tinygp_b200.kernels.quasisep import Quasisep
 from tinygp_b200.noise import Diagonal, Noise
 from tinygp_b200.solvers import DirectSolver, QuasisepSolver
@@ -42,6 +43,7 @@ class GaussianProcess:
         self.num_data = mean_value.shape[0]
         self.dtype = mean_value.dtype
         self.mean = mean_value
+        self._scalar_diag = noise is None and np.ndim(diag) == 0     # its gradient is then the sum over the diagonal
         if noise is None:  # gp.py:96-99
             diag = _default_diag(self.mean) if diag is None else diag
             noise = Diagonal(diag=_as_full_diag(diag, self.mean.shape))
@@ -70,6 +72,25 @@ class GaussianProcess:
                 loglike = -0.5 * hook(yv if self._zero_mean else yv - self.loc) - self.solver.normalization()
             return loglike if np.isfinite(loglike) else -np.inf
         return self._compute_log_prob(self._get_alpha(y))
+
+    def log_probability_and_grad(self, y) -> tuple[float, "LogProbabilityGrad"]:
+        """``log_probability(y)`` and its exact gradient with respect to the kernel parameters, the noise diagonal and
+        the mean, from one device call: the factor, L^-1 in place, and the contraction of (alpha alpha^T - K^-1) with
+        dK/dtheta evaluated tile by tile (W = K^-1 is never stored).  Needs the dense DirectSolver, a diagonal noise
+        model, and a kernel made of stationary leaves, Constant, sums, products and 0- / 1-D transforms.Linear /
+        Cholesky and Subspace, with at most 16 differentiable scalars; anything else raises NotImplementedError.  A
+        non positive-definite covariance gives (-inf, NaN gradients).  The solver's own factor is not touched."""
+        hook = getattr(self.solver, "log_probability_grad", None)
+        if hook is None:
+            raise NotImplementedError(f"log_probability_and_grad: no gradients for {type(self.solver).__name__} (only "
+                                      "the dense DirectSolver)")
+        yv = np.asarray(y, dtype=np.float64)
+        logp, grads, ddiag, alpha = hook(yv if self._zero_mean else yv - self.loc)
+        if not np.isfinite(logp):
+            logp = -np.inf
+        grad = LogProbabilityGrad(kernel=_grad_tree(self.kernel, grads, {}),
+                                  diag=float(np.sum(ddiag)) if self._scalar_diag else ddiag, mean=alpha)
+        return logp, grad
 
     def condition(self, y, X_test=None, *, diag=None, noise: Noise | None = None, include_mean: bool = True,
                   kernel=None) -> "ConditionResult":
@@ -174,6 +195,48 @@ class ConditionResult(NamedTuple):
     """gp.py:364-385"""
     log_probability: Any
     gp: GaussianProcess
+
+
+class LogProbabilityGrad(NamedTuple):
+    """Gradient of ``GaussianProcess.log_probability``: ``kernel`` is a structural copy of the kernel whose
+    differentiable fields (Constant.value, Stationary.scale, ExpSineSquared.gamma, RationalQuadratic.alpha, 0- / 1-D
+    Linear.scale and Cholesky.factor) hold d logp / d field, and whose other fields are None -- what ``jax.grad`` returns
+    for an equinox module; a node that occurs twice holds the sum.  ``diag``: d logp / d diag (a float for a scalar
+    ``diag``, else one value per point); ``mean``: d logp / d mean = K^-1 (y - mean)."""
+    kernel: Any
+    diag: Any
+    mean: np.ndarray
+
+
+def _grad_fields(node) -> tuple[str, ...]:
+    if isinstance(node, kernels.Constant):
+        return ("value",)
+    if isinstance(node, kernels.Stationary):
+        return ("scale",) + ((node.p1_field,) if node.p1_field else ())
+    if isinstance(node, transforms.Linear):
+        return ("scale",)
+    if isinstance(node, transforms.Cholesky):
+        return ("factor",)
+    return ()
+
+
+def _grad_tree(node, grads, memo):
+    if id(node) in memo:
+        return memo[id(node)]
+    out = copy.copy(node)
+    memo[id(node)] = out
+    fields = _grad_fields(node)
+    got = grads.get(id(node), (None, {}))[1]
+    for name, value in vars(node).items():
+        if isinstance(value, kernels.Kernel):
+            setattr(out, name, _grad_tree(value, grads, memo))
+        elif name in fields:
+            shape = np.shape(value)
+            g = got.get(name, np.zeros(shape) if shape else 0.0)
+            setattr(out, name, float(g) if not shape else np.asarray(g, dtype=np.float64))
+        else:
+            setattr(out, name, None)
+    return out
 
 
 def _as_full_diag(diag, shape):

@@ -39,12 +39,21 @@ class Lowering:
     MAX_METRICS = 3
     MAX_DIM = 8
 
-    def __init__(self, X=None, scalar_coords=False):
+    def __init__(self, X=None, scalar_coords=False, track=False):
         self.X = X                    # (N, D) or None when lowering without coordinates
         self.ndim0 = None if X is None else X.shape[1]   # width before any host-computed columns are appended
         self.scalar_coords = scalar_coords
         self.matrix = None            # None = untransformed coordinates
         self.metrics: list[np.ndarray] = []
+        # slot provenance, recorded when `track` is set (Kernel.lower_for_grad):
+        #   leaf_params[k] = (node, p0 field, p1 field or None) of the k-th leaf / CONST instruction, in program order;
+        #   row_owners[r] = the (node, field, index, kind) row scalings that make row r of the current matrix, kind
+        #   "linear" (row scaled by node.field[index]) or "cholesky" (scaled by 1 / node.field[index]);
+        #   metric_owners[m] = row_owners of metric m.  Metrics are shared only between leaves with the same owners.
+        self.track = track
+        self.leaf_params: list[tuple] = []
+        self.row_owners: list[tuple] | None = None
+        self.metric_owners: list[list[tuple]] = []
 
     # -- used by transform nodes ----------------------------------------------------------
     def width(self) -> int:
@@ -52,6 +61,9 @@ class Lowering:
             raise ValueError("a kernel with input transforms can only be lowered for given coordinates "
                              "(use Kernel.lower_for(X))")
         return self.X.shape[1]
+
+    def owners(self) -> list[tuple]:
+        return [()] * self.current().shape[0] if self.row_owners is None else self.row_owners
 
     def current(self) -> np.ndarray:
         return np.eye(self.ndim0, self.width()) if self.matrix is None else self.matrix
@@ -74,18 +86,26 @@ class Lowering:
         return sel
 
     # -- used by leaves -------------------------------------------------------------------
+    def note_leaf(self, node, p0_field: str, p1_field: str | None = None):
+        if self.track:
+            self.leaf_params.append((node, p0_field, p1_field))
+
     def metric_code(self) -> int:
         if self.matrix is None:
             return 0
         M = np.asarray(self.matrix, dtype=np.float64)
+        owners = self.owners() if self.track else None
         for i, other in enumerate(self.metrics):
             k = min(other.shape[1], M.shape[1])
             if other.shape[0] == M.shape[0] and np.array_equal(other[:, :k], M[:, :k]) \
-                    and not other[:, k:].any() and not M[:, k:].any():
+                    and not other[:, k:].any() and not M[:, k:].any() \
+                    and (not self.track or self.metric_owners[i] == owners):
                 return 2 * (i + 1)
         if len(self.metrics) == self.MAX_METRICS:
             raise NotImplementedError(f"at most {self.MAX_METRICS} distinct input transforms per kernel expression")
         self.metrics.append(M.copy())
+        if self.track:
+            self.metric_owners.append(owners)
         return 2 * len(self.metrics)
 
     def metric_rows(self) -> list[tuple[float, float, float, float]]:
@@ -141,6 +161,20 @@ class Kernel:
         rows = lc.metric_rows() + instr
         prog = np.ascontiguousarray(np.array(rows, dtype=np.float64).reshape(-1, _cabi.PROG_STRIDE))
         return prog, np.ascontiguousarray(lc.X)
+
+    def lower_for_grad(self, X) -> tuple[np.ndarray, np.ndarray, list[tuple], list[list[tuple]]]:
+        """``lower_for(X)`` with slot provenance: (program, coordinates, leaf_params, metric_owners) as recorded in
+        ``Lowering``.  Raises NotImplementedError for expressions without device gradients."""
+        x, scalar = _as_coords(X)
+        lc = Lowering(x, scalar, track=True)
+        instr = self.lower(lc)
+        if sum(1 for op, *_ in instr if op not in (OP_ADD, OP_MUL)) != len(lc.leaf_params):
+            raise NotImplementedError(
+                f"{type(self).__name__}: log-likelihood gradients cover stationary kernels, Constant, their sums and "
+                "products and 0- / 1-D transforms.Linear / Cholesky and Subspace; this expression holds a kernel without "
+                "a differentiable device program (e.g. a quasiseparable kernel evaluated densely)")
+        prog = np.ascontiguousarray(np.array(lc.metric_rows() + instr, dtype=np.float64).reshape(-1, _cabi.PROG_STRIDE))
+        return prog, np.ascontiguousarray(lc.X), lc.leaf_params, lc.metric_owners
 
     # -- evaluation ---------------------------------------------------------------------
     def evaluate(self, X1, X2):
@@ -245,6 +279,7 @@ class Constant(Kernel):
         self.value = float(value)
 
     def lower(self, lc):
+        lc.note_leaf(self, "value")
         return [(OP_CONST, 0, self.value, 0.0)]
 
 

@@ -19,6 +19,7 @@ from tinygp_b200.kernels.distance import Distance, L1Distance, L2Distance
 class Stationary(Kernel):
     opcode: int | None = None
     default_distance = L1Distance
+    p1_field: str | None = None     # the field behind program slot p1 (gradient provenance)
 
     def __init__(self, scale=1.0, distance: Distance | None = None):
         self.scale = scale
@@ -39,6 +40,7 @@ class Stationary(Kernel):
     def lower(self, lc):
         self._check()
         p0, p1 = self._params()
+        lc.note_leaf(self, "scale", self.p1_field)
         return [(self.opcode, self.distance.code + lc.metric_code(), p0, p1)]
 
 
@@ -71,6 +73,7 @@ class Cosine(Stationary):
 class ExpSineSquared(Stationary):
     """exp(-gamma sin^2(pi r)), stationary.py:178-205"""
     opcode = 6
+    p1_field = "gamma"
 
     def __init__(self, scale=1.0, distance: Distance | None = None, gamma=None):
         super().__init__(scale, distance)
@@ -85,6 +88,7 @@ class ExpSineSquared(Stationary):
 class RationalQuadratic(Stationary):
     """(1 + r^2 / (2 alpha))^-alpha, stationary.py:208-235"""
     opcode = 7
+    p1_field = "alpha"
 
     def __init__(self, scale=1.0, distance: Distance | None = None, alpha=None):
         super().__init__(scale, distance)

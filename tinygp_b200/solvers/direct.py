@@ -11,9 +11,12 @@ from typing import Any
 import numpy as np
 
 from tinygp_b200 import _cabi
-from tinygp_b200.kernels.base import Kernel
+from tinygp_b200.kernels.base import OP_ADD, OP_MUL, Kernel, Lowering
 from tinygp_b200.noise import Diagonal
 from tinygp_b200.solvers.solver import ConditionedCovariance, Solver
+
+
+MAX_GRAD_SLOTS = 16     # differentiable scalars per kernel program (KGRAD_MAX_SLOTS, tinygp_b200/csrc/kgrad.cuh)
 
 
 class DirectSolver(Solver):
@@ -43,6 +46,7 @@ class DirectSolver(Solver):
             if diag.shape != (x.shape[0],):
                 raise ValueError("noise diagonal must have shape (N,)")
             self._n = x.shape[0]
+            self._diag = diag
             self._x = x                      # the lowered (possibly transform-augmented) coordinates held on the device
             self.variance_value = kernel(X) + diag                              # direct.py:49
             self._cov = None
@@ -107,6 +111,60 @@ class DirectSolver(Solver):
         if self._pending is not None:
             return self._ensure(resid=y)
         return float(np.sum(np.square(self.solve_triangular(y))))
+
+    def log_probability_grad(self, resid):
+        """log_probability and its gradient for the residual ``resid = y - mean`` in one device call
+        (b200gp_dense_log_probability_grad), with a factor of its own: the solver's factor, built or pending, is left
+        as it is.  Returns (logp, grads, d logp / d diag, alpha) where ``grads`` maps id(node) to (node, {field:
+        d logp / d field}) for every kernel node with a differentiable field reached by the program."""
+        if self._x is None:
+            what = ("noise.Dense / noise.Banded" if not isinstance(self.noise, Diagonal)
+                    else "a precomputed covariance (covariance=) or a kernel without a device program")
+            raise NotImplementedError(f"log_probability_and_grad: no gradients for {what}; only kernel programs with a "
+                                      "diagonal noise model are differentiated on the device")
+        resid = _cabi.f64(resid)
+        if resid.shape != (self._n,):
+            raise ValueError("dimension mismatch")
+        prog, x, leaves, owners = self.kernel.lower_for_grad(self.X)
+        nslot = sum(2 if p1 is not None else 1 for _, _, p1 in leaves) + sum(len(o) for o in owners)
+        if nslot > MAX_GRAD_SLOTS:
+            raise NotImplementedError(f"log_probability_and_grad: the kernel has {nslot} differentiable scalars (leaf "
+                                      f"scales, constants, gamma / alpha, transform rows); at most {MAX_GRAD_SLOTS} are "
+                                      "supported")
+        logp = c_double()
+        dprog = np.zeros_like(prog)
+        dmetric = np.zeros((Lowering.MAX_METRICS, Lowering.MAX_DIM))
+        ddiag, alpha = np.empty(self._n), np.empty(self._n)
+        self._ctx.check(self._ctx.lib.b200gp_dense_log_probability_grad(
+            self._ctx.handle, _cabi.ptr(prog), prog.shape[0], _cabi.ptr(x), x.shape[0], x.shape[1], _cabi.ptr(self._diag),
+            _cabi.ptr(resid), byref(logp), _cabi.ptr(dprog), _cabi.ptr(dmetric), _cabi.ptr(ddiag), _cabi.ptr(alpha)))
+        grads: dict[int, tuple[Any, dict]] = {}
+
+        def add(node, field, value, index=None):
+            ent = grads.setdefault(id(node), (node, {}))[1]
+            shape = np.shape(getattr(node, field))
+            g = ent.setdefault(field, np.zeros(shape) if shape else 0.0)
+            if index is None or not shape:
+                ent[field] = g + value
+            else:
+                g[index] += value
+
+        n_instr = 2 * len(leaves) - 1      # leaves and the binary ADD / MUL over them, after the metric rows
+        ops, dinstr = prog[-n_instr:, 0], dprog[-n_instr:]
+        for (node, f0, f1), row in zip(leaves, np.flatnonzero((ops != OP_ADD) & (ops != OP_MUL))):
+            add(node, f0, dinstr[row, 2])
+            if f1 is not None:
+                add(node, f1, dinstr[row, 3])
+        # row-scale sensitivities R -> d/ds_r = R / s_r (Linear), -R / f_r (Cholesky); 0 where s_r = 0
+        for m, rows in enumerate(owners):
+            for r, chain in enumerate(rows):
+                R = dmetric[m, r]
+                for node, field, idx, kind in chain:
+                    v = np.asarray(getattr(node, field), dtype=np.float64)
+                    s = float(v) if v.ndim == 0 else float(v[idx])
+                    g = 0.0 if s == 0.0 else (R / s if kind == "linear" else -R / s)
+                    add(node, field, g, idx)
+        return logp.value, grads, ddiag, alpha
 
     def __del__(self):
         h = getattr(self, "_h", None)

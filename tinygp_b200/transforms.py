@@ -29,13 +29,27 @@ class _Mapped(Kernel):
     def _matrix(self, lc: Lowering) -> np.ndarray:
         raise NotImplementedError
 
+    def _rows(self, owners: list[tuple]) -> list[tuple]:
+        """row provenance (Lowering.row_owners) of this node's matrix from that of the matrix it maps"""
+        raise NotImplementedError(f"transforms.{type(self).__name__}: log-likelihood gradients cover 0- / 1-D "
+                                  "transforms.Linear / Cholesky and Subspace only")
+
     def lower(self, lc: Lowering):
-        prev = lc.matrix
+        prev, prev_owners = lc.matrix, lc.row_owners
+        if lc.track:
+            lc.row_owners = self._rows(lc.owners())
         lc.matrix = np.atleast_2d(np.asarray(self._matrix(lc), dtype=np.float64))
         try:
             return self.kernel.lower(lc)
         finally:
-            lc.matrix = prev
+            lc.matrix, lc.row_owners = prev, prev_owners
+
+
+def _scaled_rows(node, field: str, kind: str, owners: list[tuple]) -> list[tuple]:
+    v = np.asarray(getattr(node, field))
+    if v.ndim >= 2:
+        return _Mapped._rows(node, owners)
+    return [o + ((node, field, r if v.ndim == 1 else 0, kind),) for r, o in enumerate(owners)]
 
 
 class Transform(_Mapped):
@@ -69,6 +83,9 @@ class Linear(_Mapped):
             return scale @ cur
         raise ValueError("'scale' must be 0-, 1-, or 2-dimensional")
 
+    def _rows(self, owners):
+        return _scaled_rows(self, "scale", "linear", owners)
+
 
 class Cholesky(_Mapped):
     """transforms.py:77-136 -- ``X / factor`` for 0-/1-D ``factor``, ``solve_triangular(factor, X, lower=True)``
@@ -91,6 +108,9 @@ class Cholesky(_Mapped):
                 out[i] = (cur[i] - L[i, :i] @ out[:i]) / L[i, i]
             return out
         raise ValueError("'scale' must be 0-, 1-, or 2-dimensional")
+
+    def _rows(self, owners):
+        return _scaled_rows(self, "factor", "cholesky", owners)
 
     @classmethod
     def from_parameters(cls, diagonal, off_diagonal, kernel: Kernel) -> "Cholesky":
@@ -120,3 +140,6 @@ class Subspace(_Mapped):
         cur = lc.current()
         axis = self.axis if np.ndim(self.axis) == 0 else list(self.axis)
         return cur[axis]
+
+    def _rows(self, owners):
+        return [owners[a] for a in np.atleast_1d(self.axis)]
