@@ -104,9 +104,13 @@ typedef struct {
 } b200gp_profile;
 int b200gp_get_profile(b200gp_ctx* ctx, b200gp_profile* out, int reset);
 
-/* fp64 tensor (DMMA) peak micro-benchmark on this device: returns achieved TFLOP/s of a
- * register-resident mma.sync.m8n8k4.f64 loop on all SMs, and of a DFMA loop. */
+/* fp64 tensor (DMMA) peak micro-benchmark on this device: returns achieved TFLOP/s of a register-resident loop, on
+ * all SMs, of the mma shape the fp64 GEMM mainloops issue (mma.sync.m16n8k16.f64), and of a DFMA loop.
+ * The loop length is the option "peak_iters", in units of 16 m8n8k4 instructions per warp (equal flops for every shape). */
 int b200gp_measure_fp64_peak(b200gp_ctx* ctx, double* dmma_tflops, double* dfma_tflops);
+/* the same DMMA loop for one fp64 mma shape (m, n, k): (8, 8, 4), (16, 8, 4), (16, 8, 8) or (16, 8, 16); TFLOP/s
+ * counting 2 m n k flop per instruction.  For measurement only (tools/dmma_shapes.py). */
+int b200gp_measure_dmma_shape(b200gp_ctx* ctx, int m, int n, int k, double* tflops);
 /* int8 tensor peak micro-benchmark: wgmma.m64n128k32.s32.s8.s8 issued back to back by two warpgroups on every SM
  * from resident shared-memory operands (no TMA traffic); returns TOP/s (2 x MAC). */
 int b200gp_measure_i8_peak(b200gp_ctx* ctx, double* tops);

@@ -49,6 +49,7 @@ SIGNATURES = {
     "b200gp_get_option": (c_int, [c_void_p, c_char_p, POINTER(c_int64)]),
     "b200gp_get_profile": (c_int, [c_void_p, POINTER(Profile), c_int]),
     "b200gp_measure_fp64_peak": (c_int, [c_void_p, c_double_p, c_double_p]),
+    "b200gp_measure_dmma_shape": (c_int, [c_void_p, c_int, c_int, c_int, c_double_p]),
     "b200gp_measure_i8_peak": (c_int, [c_void_p, c_double_p]),
     "b200gp_i8_update_test": (c_int, [_V, _D, _I, _L, _L, _D, _D]),
     "b200gp_i8_update_bench": (c_int, [_V, _L, _L, _L, _I, _I, _L, _L, c_double_p, c_void_p]),
@@ -197,6 +198,11 @@ class Context:
         a, b = c_double(), c_double()
         self.check(self.lib.b200gp_measure_fp64_peak(self.handle, byref(a), byref(b)))
         return a.value, b.value
+
+    def measure_dmma_shape(self, m: int, n: int, k: int) -> float:
+        t = c_double()
+        self.check(self.lib.b200gp_measure_dmma_shape(self.handle, m, n, k, byref(t)))
+        return t.value
 
     def measure_i8_peak(self):
         a = c_double()

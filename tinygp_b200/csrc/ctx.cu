@@ -1,6 +1,8 @@
 // Context, device-buffer cache, options, profile counters and the fp64 peak micro-benchmarks.
 #include "common.cuh"
+#include "dmma.cuh"
 #include <string.h>
+#include <algorithm>
 
 void* b200gp_ctx::alloc(size_t bytes) {
     if (bytes == 0) bytes = 8;
@@ -80,21 +82,49 @@ void b200gp_ctx::trim() {
 }
 
 // ---- fp64 peak micro-benchmarks ----------------------------------------------------------------
+// one mma.sync.MxNxK.f64 (N = 8): M = 8, K = 4 (Ampere's shape) or M = 16, K = 4 / 8 / 16 (sm_90)
+template <int M, int K>
+__device__ __forceinline__ void peak_mma(double (&c)[M / 4], const double (&a)[M * K / 32], const double (&b)[K / 4]) {
+    if constexpr (M == 8)
+        asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
+                     : "+d"(c[0]), "+d"(c[1]) : "d"(a[0]), "d"(b[0]));
+    else if constexpr (K == 4)
+        asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+                     : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3]) : "d"(a[0]), "d"(a[1]), "d"(b[0]));
+    else if constexpr (K == 8)
+        asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, "
+                     "{%0,%1,%2,%3};\n"
+                     : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+                     : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(b[0]), "d"(b[1]));
+    else
+        asm volatile("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, "
+                     "{%12,%13,%14,%15}, {%0,%1,%2,%3};\n"
+                     : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+                     : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]),
+                       "d"(b[0]), "d"(b[1]), "d"(b[2]), "d"(b[3]));
+}
+
+// register-resident operands, 16 independent accumulators per warp, `iters` rounds of 16 instructions
+template <int M, int K>
 __global__ void __launch_bounds__(256) dmma_peak_kernel(double* out, int iters) {
-    double c[16][2];
+    double c[16][M / 4], a[M * K / 32], b[K / 4];
 #pragma unroll
-    for (int i = 0; i < 16; ++i) c[i][0] = c[i][1] = 0.0;
-    double a = 1.0 + threadIdx.x * 1e-9, b = 1.0 - threadIdx.x * 1e-9;
+    for (int i = 0; i < 16; ++i)
+#pragma unroll
+        for (int j = 0; j < M / 4; ++j) c[i][j] = 0.0;
+#pragma unroll
+    for (int j = 0; j < M * K / 32; ++j) a[j] = 1.0 + (threadIdx.x + j) * 1e-9;
+#pragma unroll
+    for (int j = 0; j < K / 4; ++j) b[j] = 1.0 - (threadIdx.x + j) * 1e-9;
     for (int it = 0; it < iters; ++it) {
 #pragma unroll
-        for (int i = 0; i < 16; ++i)
-            asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
-                         : "+d"(c[i][0]), "+d"(c[i][1])
-                         : "d"(a), "d"(b));
+        for (int i = 0; i < 16; ++i) peak_mma<M, K>(c[i], a, b);
     }
     double s = 0.0;
 #pragma unroll
-    for (int i = 0; i < 16; ++i) s += c[i][0] + c[i][1];
+    for (int i = 0; i < 16; ++i)
+#pragma unroll
+        for (int j = 0; j < M / 4; ++j) s += c[i][j];
     out[blockIdx.x * blockDim.x + threadIdx.x] = s;
 }
 
@@ -259,21 +289,45 @@ int b200gp_get_profile(b200gp_ctx* ctx, b200gp_profile* out, int reset) {
     API_END
 }
 
+// TFLOP/s of dmma_peak_kernel<M, K> on all SMs, timed after one warm-up launch.  peak_iters counts work in units of
+// 16 m8n8k4 instructions per warp, so every shape runs the same flop count.
+static double dmma_shape_tflops(b200gp_ctx* ctx, int m, int k, double* buf, int blocks, int threads) {
+    const int iters = (int)std::max<int64_t>(1, ctx->peak_iters * 8 * 4 / (m * k));
+    float ms = 0;
+    for (int rep = 0; rep < 2; ++rep) {  // first pass warms up
+        cudaEventRecord(ctx->ev0, ctx->stream);
+        if (m == 8) dmma_peak_kernel<8, 4><<<blocks, threads, 0, ctx->stream>>>(buf, iters);
+        else if (k == 4) dmma_peak_kernel<16, 4><<<blocks, threads, 0, ctx->stream>>>(buf, iters);
+        else if (k == 8) dmma_peak_kernel<16, 8><<<blocks, threads, 0, ctx->stream>>>(buf, iters);
+        else dmma_peak_kernel<16, 16><<<blocks, threads, 0, ctx->stream>>>(buf, iters);
+        cudaEventRecord(ctx->ev1, ctx->stream);
+        CUDA_CHECK(cudaEventSynchronize(ctx->ev1));
+        cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
+    }
+    ctx->launches += 2;
+    // per warp per instruction: m * 8 * k FMA = 2 m 8 k flop
+    return (double)blocks * (threads / 32) * (double)iters * 16.0 * (2.0 * m * 8 * k) / (ms * 1e-3) / 1e12;
+}
+
+int b200gp_measure_dmma_shape(b200gp_ctx* ctx, int m, int n, int k, double* tflops) {
+    API_BEGIN(ctx)
+    if (!tflops) throw GpError("measure_dmma_shape: null output");
+    if (n != 8 || !((m == 8 && k == 4) || (m == 16 && (k == 4 || k == 8 || k == 16))))
+        throw GpError("measure_dmma_shape: the fp64 mma shapes are m8n8k4, m16n8k4, m16n8k8 and m16n8k16");
+    const int blocks = _ctx->num_sms * 4, threads = 256;
+    double* buf = (double*)_ctx->alloc((size_t)blocks * threads * 8);
+    *tflops = dmma_shape_tflops(_ctx, m, k, buf, blocks, threads);
+    _ctx->release(buf, (size_t)blocks * threads * 8);
+    API_END
+}
+
 int b200gp_measure_fp64_peak(b200gp_ctx* ctx, double* dmma_tflops, double* dfma_tflops) {
     API_BEGIN(ctx)
     const int blocks = _ctx->num_sms * 4, threads = 256;
     const int iters = (int)_ctx->peak_iters;
     double* buf = (double*)_ctx->alloc((size_t)blocks * threads * 8);
+    *dmma_tflops = dmma_shape_tflops(_ctx, 16, dmma::MK, buf, blocks, threads);   // the shape the GEMM mainloops issue
     float ms = 0;
-    for (int rep = 0; rep < 2; ++rep) {  // first pass warms up
-        cudaEventRecord(_ctx->ev0, _ctx->stream);
-        dmma_peak_kernel<<<blocks, threads, 0, _ctx->stream>>>(buf, iters);
-        cudaEventRecord(_ctx->ev1, _ctx->stream);
-        CUDA_CHECK(cudaEventSynchronize(_ctx->ev1));
-        cudaEventElapsedTime(&ms, _ctx->ev0, _ctx->ev1);
-    }
-    // per warp per instruction: 8*8*4 FMA = 512 flop
-    *dmma_tflops = (double)blocks * (threads / 32) * (double)iters * 16.0 * 512.0 / (ms * 1e-3) / 1e12;
     for (int rep = 0; rep < 2; ++rep) {
         cudaEventRecord(_ctx->ev0, _ctx->stream);
         dfma_peak_kernel<<<blocks, threads, 0, _ctx->stream>>>(buf, iters);
@@ -282,7 +336,7 @@ int b200gp_measure_fp64_peak(b200gp_ctx* ctx, double* dmma_tflops, double* dfma_
         cudaEventElapsedTime(&ms, _ctx->ev0, _ctx->ev1);
     }
     *dfma_tflops = (double)blocks * threads * (double)iters * 16.0 * 2.0 / (ms * 1e-3) / 1e12;
-    _ctx->launches += 4;
+    _ctx->launches += 2;
     _ctx->release(buf, (size_t)blocks * threads * 8);
     API_END
 }

@@ -1,5 +1,5 @@
 // Dense DirectSolver path for sm_90a: pairwise kernel build (K1), blocked right-looking Cholesky
-// whose panel/trailing updates run on the fp64 tensor pipe (DMMA, mma.sync.m8n8k4.f64) (K2),
+// whose panel/trailing updates run on the fp64 tensor pipe (DMMA, mma.sync.m16n8k16.f64, dmma.cuh) (K2),
 // triangular solves + reductions behind log_probability (K3), L@z (K4).
 //
 // Reference behaviour being replaced: src/tinygp/solvers/direct.py:30-95 (DirectSolver),
@@ -9,8 +9,9 @@
 // Data layout in HBM: one np x np row-major fp64 matrix (np = n rounded up to 128; the pad is an
 // identity block so it contributes log 1 = 0 to the determinant), lower triangle significant.
 // Row-major makes BOTH operands of every update  C_ij -= P_i P_j^T  K-contiguous (a panel row is
-// a contiguous run of doubles), which is exactly the row.col operand form of mma.m8n8k4.f64.
+// a contiguous run of doubles), which is exactly the row.col operand form of mma.m16n8k16.f64.
 #include "common.cuh"
+#include "dmma.cuh"
 #include <limits.h>
 
 // =============================================================================================
@@ -306,13 +307,11 @@ void dense_build_rect(b200gp_ctx* ctx, const KProg& prog, const double* X1, int6
 
 // =============================================================================================
 // K2 core: NT GEMM on the fp64 tensor pipe.   C (op)= alpha * A(MxK) * B(NxK)^T
-// 128x128 CTA tile, 8 warps (2 x 4), warp tile 64 x 32 = 8 x 4 DMMA m8n8k4 atoms,
+// 128x128 CTA tile, 8 warps (2 x 4), warp tile 64 x 32 = 4 x 4 DMMA m16n8k16 atoms (dmma.cuh),
 // BK = 16 doubles (one 128-byte line per row per stage), 4-stage cp.async pipeline.
-// Shared-memory rows are padded 16 -> 20 doubles so that the (8 rows x 4 k) fragment loads of a
-// half-warp hit 16 distinct 8-byte bank pairs (row stride 40 words = 8 mod 32).
 // =============================================================================================
 namespace gemm {
-constexpr int BM = 128, BN = 128, BK = 16, STAGES = 4, LDS = 20, THREADS = 256;
+constexpr int BM = 128, BN = 128, BK = dmma::BK, STAGES = 4, LDS = dmma::LDS, THREADS = 256;
 constexpr int STAGE_DOUBLES = (BM + BN) * LDS;
 constexpr int SMEM_BYTES = STAGES * STAGE_DOUBLES * (int)sizeof(double);  // 163840
 constexpr int BAND = 16;  // tile rows per rasterisation band (L2 reuse of the panel operands)
@@ -338,12 +337,6 @@ __device__ __forceinline__ void cp_async16(void* smem_ptr, const void* gptr) {
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
-
-__device__ __forceinline__ void dmma884(double& c0, double& c1, const double a, const double b) {
-    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
-                 : "+d"(c0), "+d"(c1)
-                 : "d"(a), "d"(b));
-}
 
 // linear CTA index -> lower-triangular tile (ti, tj), banded so that concurrently resident CTAs
 // share 16 A row-panels and a handful of B row-panels (both stay in L2).
@@ -377,7 +370,6 @@ template <bool LOWER>
 __global__ void __launch_bounds__(THREADS, 1) gemm_nt_kernel(const __grid_constant__ KProg P, const Args g) {
     extern __shared__ __align__(16) double smem[];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int gq = lane >> 2, tq = lane & 3;
     const int wm = warp >> 2, wn = warp & 3;
 
     int ti, tj;
@@ -424,32 +416,21 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_nt_kernel(const __grid_consta
         const int nk = kc + STAGES - 1;
         if (nk < KT) load_stage(nk % STAGES, nk);
         cp_async_commit();
-        const double* as = smem + (kc % STAGES) * STAGE_DOUBLES + (wm * 64 + gq) * LDS + tq;
-        const double* bs = smem + (kc % STAGES) * STAGE_DOUBLES + BM * LDS + (wn * 32 + gq) * LDS + tq;
-#pragma unroll
-        for (int kk = 0; kk < BK / 4; ++kk) {
-            double a[8], b[4];
-#pragma unroll
-            for (int mi = 0; mi < 8; ++mi) a[mi] = as[mi * 8 * LDS + kk * 4];
-#pragma unroll
-            for (int ni = 0; ni < 4; ++ni) b[ni] = bs[ni * 8 * LDS + kk * 4];
-#pragma unroll
-            for (int mi = 0; mi < 8; ++mi)
-#pragma unroll
-                for (int ni = 0; ni < 4; ++ni) dmma884(acc[mi][ni][0], acc[mi][ni][1], a[mi], b[ni]);
-        }
+        const double* as = smem + (kc % STAGES) * STAGE_DOUBLES + wm * dmma::WM * LDS;
+        const double* bs = smem + (kc % STAGES) * STAGE_DOUBLES + BM * LDS + wn * dmma::WN * LDS;
+        dmma::warp_tile_stage(acc, as, bs, lane);
     }
 
-    // epilogue: thread owns rows (wm*64 + mi*8 + gq), column pairs (wn*32 + ni*8 + 2*tq)
-    const int64_t crow0 = (int64_t)ti * BM + wm * 64 + gq;
-    const int64_t ccol0 = (int64_t)tj * BN + wn * 32 + 2 * tq;
+    // epilogue: acc[mi][ni][q] is C(row0 + acc_row(mi), col0 + acc_col(ni, q)); q = 0, 1 are adjacent columns
+    const int64_t crow0 = (int64_t)ti * BM + wm * dmma::WM;
+    const int64_t ccol0 = (int64_t)tj * BN + wn * dmma::WN;
 #pragma unroll
     for (int mi = 0; mi < 8; ++mi) {
-        const int64_t r = crow0 + mi * 8;
+        const int64_t r = crow0 + dmma::acc_row(lane, mi);
         double* crow = g.C + bz * g.strideC + r * g.ldc;
 #pragma unroll
         for (int ni = 0; ni < 4; ++ni) {
-            const int64_t c = ccol0 + ni * 8;
+            const int64_t c = ccol0 + dmma::acc_col(lane, ni, 0);
             double2 v;
             if (g.beta_mode == 1) {
                 v = *reinterpret_cast<const double2*>(crow + c);

@@ -13,11 +13,12 @@
 // Extra device memory: O(n) vectors, 128 x np for the transposed diagonal blocks and the block-column operand, and
 // tiles x 16 partial sums.  No second np x np buffer.
 #include "common.cuh"
+#include "dmma.cuh"
 #include "kgrad.cuh"
 #include <limits.h>
 
 namespace tg {
-constexpr int BM = 128, BK = 16, STAGES = 4, LDS = 20, THREADS = 256;
+constexpr int BM = 128, BK = dmma::BK, STAGES = 4, LDS = dmma::LDS, THREADS = 256;
 constexpr int STAGE_DOUBLES = 2 * BM * LDS;
 constexpr int SMEM_BYTES = STAGES * STAGE_DOUBLES * (int)sizeof(double);   // 163840 (>= the 128 x 128 W tile)
 constexpr int CHUNKS = TILE / BK;                                           // K chunks per 128-block
@@ -52,11 +53,6 @@ __device__ __forceinline__ void cp_async16(void* smem_ptr, const void* gptr) {
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
-__device__ __forceinline__ void dmma884(double& c0, double& c1, const double a, const double b) {
-    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
-                 : "+d"(c0), "+d"(c1)
-                 : "d"(a), "d"(b));
-}
 
 __device__ __forceinline__ const double* block_ptr(const double* base, int64_t ld, const double* diag, int rowblk, int kblk,
                                                    int64_t& ldo) {
@@ -68,12 +64,11 @@ __device__ __forceinline__ const double* block_ptr(const double* base, int64_t l
     return base + (int64_t)rowblk * TILE * ld + (int64_t)kblk * TILE;
 }
 
-// 128 x 128 CTA tile, 8 warps (2 x 4) of 64 x 32, mma.sync.m8n8k4.f64, 4-stage cp.async pipeline (the layout of
-// dense.cu's gemm_nt_kernel) over a per-tile K range of 128-blocks
+// 128 x 128 CTA tile, 8 warps (2 x 4) of 64 x 32, the DMMA warp tile of dmma.cuh (mma.sync.m16n8k16.f64), 4-stage
+// cp.async pipeline (the layout of dense.cu's gemm_nt_kernel) over a per-tile K range of 128-blocks
 __global__ void __launch_bounds__(THREADS, 1) tri_gemm_kernel(const __grid_constant__ Args g) {
     extern __shared__ __align__(16) double smem[];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int gq = lane >> 2, tq = lane & 3;
     const int wm = warp >> 2, wn = warp & 3;
     int ti, tj, klo, khi;
     if (g.mode == PANEL) {
@@ -126,32 +121,21 @@ __global__ void __launch_bounds__(THREADS, 1) tri_gemm_kernel(const __grid_const
         const int nk = kc + STAGES - 1;
         if (nk < KT) load_stage(nk % STAGES, nk);
         cp_async_commit();
-        const double* as = smem + (kc % STAGES) * STAGE_DOUBLES + (wm * 64 + gq) * LDS + tq;
-        const double* bs = smem + (kc % STAGES) * STAGE_DOUBLES + BM * LDS + (wn * 32 + gq) * LDS + tq;
-#pragma unroll
-        for (int kk = 0; kk < BK / 4; ++kk) {
-            double a[8], b[4];
-#pragma unroll
-            for (int mi = 0; mi < 8; ++mi) a[mi] = as[mi * 8 * LDS + kk * 4];
-#pragma unroll
-            for (int ni = 0; ni < 4; ++ni) b[ni] = bs[ni * 8 * LDS + kk * 4];
-#pragma unroll
-            for (int mi = 0; mi < 8; ++mi)
-#pragma unroll
-                for (int ni = 0; ni < 4; ++ni) dmma884(acc[mi][ni][0], acc[mi][ni][1], a[mi], b[ni]);
-        }
+        const double* as = smem + (kc % STAGES) * STAGE_DOUBLES + wm * dmma::WM * LDS;
+        const double* bs = smem + (kc % STAGES) * STAGE_DOUBLES + BM * LDS + wn * dmma::WN * LDS;
+        dmma::warp_tile_stage(acc, as, bs, lane);
     }
     cp_async_wait<0>();
 
     if (g.mode != CONTRACT) {
-        const int64_t crow0 = (int64_t)ti * BM + wm * 64 + gq;
-        const int64_t ccol0 = (int64_t)tj * BM + wn * 32 + 2 * tq;
+        const int64_t crow0 = (int64_t)ti * BM + wm * dmma::WM;
+        const int64_t ccol0 = (int64_t)tj * BM + wn * dmma::WN;
 #pragma unroll
         for (int mi = 0; mi < 8; ++mi) {
-            double* crow = g.C + (crow0 + mi * 8) * g.ldc;
+            double* crow = g.C + (crow0 + dmma::acc_row(lane, mi)) * g.ldc;
 #pragma unroll
             for (int ni = 0; ni < 4; ++ni)
-                *reinterpret_cast<double2*>(crow + ccol0 + ni * 8) =
+                *reinterpret_cast<double2*>(crow + ccol0 + dmma::acc_col(lane, ni, 0)) =
                     make_double2(g.alpha * acc[mi][ni][0], g.alpha * acc[mi][ni][1]);
         }
         return;
@@ -164,7 +148,7 @@ __global__ void __launch_bounds__(THREADS, 1) tri_gemm_kernel(const __grid_const
     for (int mi = 0; mi < 8; ++mi)
 #pragma unroll
         for (int ni = 0; ni < 4; ++ni) {
-            const int r = wm * 64 + mi * 8 + gq, c = wn * 32 + ni * 8 + 2 * tq;
+            const int r = wm * dmma::WM + dmma::acc_row(lane, mi), c = wn * dmma::WN + dmma::acc_col(lane, ni, 0);
             Ws[r * BM + c] = acc[mi][ni][0];
             Ws[r * BM + c + 1] = acc[mi][ni][1];
         }
