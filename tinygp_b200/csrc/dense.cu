@@ -315,6 +315,7 @@ constexpr int BM = 128, BN = 128, BK = dmma::BK, STAGES = 4, LDS = dmma::LDS, TH
 constexpr int STAGE_DOUBLES = (BM + BN) * LDS;
 constexpr int SMEM_BYTES = STAGES * STAGE_DOUBLES * (int)sizeof(double);  // 163840
 constexpr int BAND = 16;  // tile rows per rasterisation band (L2 reuse of the panel operands)
+constexpr int C_PREFETCH = 4;   // stages before the end of K at which a beta_mode 1 tile of C is prefetched into L2
 
 struct Args {
     const double* A; int64_t lda;
@@ -416,6 +417,15 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_nt_kernel(const __grid_consta
         const int nk = kc + STAGES - 1;
         if (nk < KT) load_stage(nk % STAGES, nk);
         cp_async_commit();
+        if (g.beta_mode == 1 && kc == (KT > C_PREFETCH ? KT - C_PREFETCH : 0)) {
+            // the C tile (128 rows x 8 lines of 128 B) into L2, so that the epilogue's reads do not wait on HBM
+#pragma unroll
+            for (int i = 0; i < BM * BN / 16 / THREADS; ++i) {
+                const int line = tid + i * THREADS;
+                const double* p = g.C + bz * g.strideC + ((int64_t)ti * BM + (line >> 3)) * g.ldc + (int64_t)tj * BN + (line & 7) * 16;
+                asm volatile("prefetch.global.L2 [%0];\n" ::"l"(p));
+            }
+        }
         const double* as = smem + (kc % STAGES) * STAGE_DOUBLES + wm * dmma::WM * LDS;
         const double* bs = smem + (kc % STAGES) * STAGE_DOUBLES + BM * LDS + wn * dmma::WN * LDS;
         dmma::warp_tile_stage(acc, as, bs, lane);
@@ -424,6 +434,32 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_nt_kernel(const __grid_consta
     // epilogue: acc[mi][ni][q] is C(row0 + acc_row(mi), col0 + acc_col(ni, q)); q = 0, 1 are adjacent columns
     const int64_t crow0 = (int64_t)ti * BM + wm * dmma::WM;
     const int64_t ccol0 = (int64_t)tj * BN + wn * dmma::WN;
+    if (g.beta_mode == 1) {
+        // C += alpha AB.  Two accumulator rows' reads are issued before any of their writes: one read-write round trip
+        // per element would serialise 32 memory latencies per thread (the compiler cannot move a read of C above a
+        // write to C).
+#pragma unroll
+        for (int mi = 0; mi < 8; mi += 2) {
+            double* crow[2];
+            double2 v[2][4];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                crow[h] = g.C + bz * g.strideC + (crow0 + dmma::acc_row(lane, mi + h)) * g.ldc;
+#pragma unroll
+                for (int ni = 0; ni < 4; ++ni)
+                    v[h][ni] = *reinterpret_cast<const double2*>(crow[h] + ccol0 + dmma::acc_col(lane, ni, 0));
+            }
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int ni = 0; ni < 4; ++ni) {
+                    v[h][ni].x += g.alpha * acc[mi + h][ni][0];
+                    v[h][ni].y += g.alpha * acc[mi + h][ni][1];
+                    *reinterpret_cast<double2*>(crow[h] + ccol0 + dmma::acc_col(lane, ni, 0)) = v[h][ni];
+                }
+        }
+        return;
+    }
 #pragma unroll
     for (int mi = 0; mi < 8; ++mi) {
         const int64_t r = crow0 + dmma::acc_row(lane, mi);
@@ -432,9 +468,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_nt_kernel(const __grid_consta
         for (int ni = 0; ni < 4; ++ni) {
             const int64_t c = ccol0 + dmma::acc_col(lane, ni, 0);
             double2 v;
-            if (g.beta_mode == 1) {
-                v = *reinterpret_cast<const double2*>(crow + c);
-            } else if (g.beta_mode == 2) {
+            if (g.beta_mode == 2) {
                 const int64_t gr = g.row0 + r;
                 double e[2];
 #pragma unroll
