@@ -78,7 +78,6 @@ const char* b200gp_last_error(b200gp_ctx* ctx);
 /* number of kernel launches issued by this context since creation (bench "gpu_launches"). */
 int64_t b200gp_launch_count(b200gp_ctx* ctx);
 /* tunables: "nb" (outer panel width, multiple of 128), "profile" (0/1: per-kernel CUDA-event timers),
- * "panel_overlap" (0/1: inside a panel, update the rows below the diagonal tile on a side stream while potf2 runs),
  * "build_ahead" (0/1: generate block column J+1 on a side stream under the int8 update of column J),
  * "qs_chunk" (points per thread in the quasiseparable scans), "qs_tree" (0: thread-sequential fan-in-16 tree over the
  * chunk composites, 1: warp-shuffle scan kernels, fan-in 32) */

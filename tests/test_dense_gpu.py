@@ -63,27 +63,23 @@ def test_scalar_evaluate_and_edge_shapes():
         k(np.zeros((0,)), np.zeros((3,)))
 
 
-@pytest.mark.parametrize("potf2", [2, 1])
+@pytest.mark.parametrize("nb", [128, 512, 1024])   # n = 1100 at nb 512 / 1024: the last panel is 128 columns wide
 @pytest.mark.parametrize("n", [1, 50, 128, 300, 1100])
-def test_factor_parity(n, ctx, potf2):
-    ctx.set_option("potf2_version", potf2)
+def test_factor_parity(n, nb, ctx):
     rng = np.random.default_rng(n)
     X = rng.uniform(0, 6, (n, 2))
     k = 1.3 * kernels.ExpSquared(0.8)
     diag = rng.uniform(0.05, 0.2, n)
-    for nb in (128, 512):
-        ctx.set_option("nb", nb)
-        ctx.set_option("ozaki_slices", 0)      # the native fp64 DMMA path is the one under test here
-        s = solvers.DirectSolver(k, X, noise.Diagonal(diag))
-        so = o.DirectSolver(to_oracle(k), X, o.Diagonal(diag))
-        assert s.info == 0
-        np.testing.assert_allclose(s.scale_tril, so.scale_tril, rtol=1e-10, atol=1e-12)
-        assert rel(s.normalization(), so.normalization()) < 1e-12
-        assert_close(s.variance(), so.variance(), 1e-14, 1e-14)
-        np.testing.assert_allclose(s.covariance(), so.covariance(), rtol=1e-13, atol=1e-15)
-    ctx.set_option("nb", 1024)
+    ctx.set_option("nb", nb)
+    ctx.set_option("ozaki_slices", 0)      # the native fp64 DMMA path is the one under test here
+    s = solvers.DirectSolver(k, X, noise.Diagonal(diag))
+    so = o.DirectSolver(to_oracle(k), X, o.Diagonal(diag))
+    assert s.info == 0
+    np.testing.assert_allclose(s.scale_tril, so.scale_tril, rtol=1e-10, atol=1e-12)
+    assert rel(s.normalization(), so.normalization()) < 1e-12
+    assert_close(s.variance(), so.variance(), 1e-14, 1e-14)
+    np.testing.assert_allclose(s.covariance(), so.covariance(), rtol=1e-13, atol=1e-15)
     ctx.reset_options()       # library defaults (NOT a literal: the default plane count is 7)
-    ctx.set_option("potf2_version", 2)
 
 
 @pytest.mark.parametrize("n,ndim,name", [(256, 1, "expsq"), (777, 3, "c3_l2"), (2048, 3, "expsq"),

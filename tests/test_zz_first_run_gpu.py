@@ -2,7 +2,7 @@
 under `pytest -x`:
   * QuasisepSolver conditioning on the device (`b200gp_qs_condition`), diag((K + N)^-1) and the O(N) conditioned variance
     (GramBack backward scan; its source passes on the CPU in tests/test_device_code_on_host.py);
-  * the K-range split of the int8 update, the panel-overlap / build-ahead options, the warp-shuffle tree option;
+  * the K-range split of the int8 update, the build-ahead option, the warp-shuffle tree option;
 The reference-golden / restated-reference cases that depend on this code follow in test_zzy_*, the changed and new int8
 kernel variants in test_zzz_*."""
 
@@ -131,32 +131,27 @@ def test_int8_update_splits_k_ranges_beyond_the_int32_bound(ctx):
     np.testing.assert_allclose(got, want, rtol=0, atol=1e-12 * max(1.0, np.abs(want).max()))
 
 
-@pytest.mark.parametrize("slices", [0, 7])
-def test_panel_overlap_option_gives_the_same_factorisation(ctx, slices):
-    """options panel_overlap (inside a panel the rows below the diagonal tile are updated on a side stream while potf2
-    runs) and build_ahead (block column J+1 is generated on a side stream under the int8 update of column J): pure
-    reorderings of independent work, so the results must be bit-identical to the serial order"""
+@pytest.mark.parametrize("n", [3000, 2600])         # nb = 512: six full panels; five and a last one of 128 columns
+def test_build_ahead_option_gives_the_same_factorisation(ctx, n):
+    """option build_ahead (block column J+1 is generated on a side stream under the int8 update of column J): a pure
+    reordering of independent work, so the result must be bit-identical to the serial order"""
     from tinygp_b200 import kernels
-    n = 3000
     rng = np.random.default_rng(17)
     X = rng.uniform(0, 20.0 * (n / 65536.0) ** (1 / 3), (n, 3))
     y = np.sin(X[:, 0]) + 0.1 * rng.normal(size=n)
     k = 1.3 * kernels.ExpSquared(0.8)
     ctx.set_option("nb", 512)
-    ctx.set_option("ozaki_min_n", 0 if slices else 1 << 40)
-    ctx.set_option("ozaki_slices", slices if slices else 7)
+    ctx.set_option("ozaki_min_n", 0)
+    ctx.set_option("ozaki_slices", 7)
     out = []
     try:
         ctx.set_option("ozaki_subpanel", 0)      # one fp64 panel per block column: 4 diagonal tiles per look-ahead chain
-        ctx.set_option("panel_chain", 0)         # left-looking chain: the order of the serial panel (the default right-looking
-                                                 # chain sums the diagonal block differently: test_zzz_*::test_right_looking_*)
-        for overlap, ahead in ((0, 0), (1, 0), (0, 1), (1, 1), (2, 0), (2, 1)):
-            ctx.set_option("panel_overlap", overlap)   # 2 = look-ahead: diagonal block on the main stream, rows below on a side stream
+        for ahead in (0, 1):
             ctx.set_option("build_ahead", ahead)
             out.append(GaussianProcess(k, X, diag=0.1).log_probability(y))
     finally:
         ctx.reset_options()
-    assert all(v == out[0] for v in out), out
+    assert out[0] == out[1], out
     lpo = o.GaussianProcess(to_oracle(k), X, diag=0.1).log_probability(y)
     assert rel(out[0], lpo) < LOGP_RTOL
 

@@ -1,5 +1,6 @@
 """One factorisation sharded over TWO GPUs (NCCL, one process per GPU): BASELINE config 3's path at a size the oracle
-can check.  Skipped when fewer than two CUDA devices are visible (the driver's 1-GPU test box)."""
+can check; skipped when fewer than two CUDA devices are visible.  The split panel step of the sharded path
+(b200gp_mg_panel_factor / b200gp_mg_panel_finish) is also driven with one rank, which needs one GPU only."""
 
 import os
 import socket
@@ -87,3 +88,44 @@ def test_sharded_two_ranks_matches_oracle_and_single_rank(streaming, split, mg_s
         assert lp1 == res[0][1], (lp1, res)
     else:
         assert abs(lp1 - res[0][1]) <= 1e-12 * abs(lp1), (lp1, res)
+
+
+@pytest.mark.parametrize("n,last", [(1100, 128), (1536, 512)])
+def test_split_panel_step_on_one_rank(ctx, n, last):
+    """b200gp_mg_panel_factor (diagonal block + this rank's rows below it) then b200gp_mg_panel_finish, with world = 1:
+    bit-identical to the one-call panel step b200gp_mg_panel, and parity with the oracle.  nb = 512: n = 1100 ends with a
+    128-column panel, n = 1536 has three full ones."""
+    from ctypes import byref, c_double, c_int, c_int64, c_void_p
+    from oracle import tinygp_np as o
+    from tinygp_b200 import _cabi, kernels, multigpu
+    from util import LOGP_RTOL, rel, to_oracle
+    rng = np.random.default_rng(n)
+    X = np.ascontiguousarray(rng.uniform(0, 20.0 * (n / 65536.0) ** (1 / 3), (n, 3)))
+    y = np.sin(X[:, 0]) + 0.1 * rng.normal(size=n)
+    diag = np.full(n, 0.1)
+    k = 1.3 * kernels.ExpSquared(0.8)
+    ctx.set_option("nb", 512)
+    prog, x = k.lower_for(X)
+    d, r = _cabi.f64(diag), _cabi.f64(y)
+    lib = ctx.lib
+    mg = c_void_p()
+    ctx.check(lib.b200gp_mg_create(ctx.handle, _cabi.ptr(prog), prog.shape[0], _cabi.ptr(x), n, x.shape[1], _cabi.ptr(d),
+                                   _cabi.ptr(r), 7, 0, byref(mg)))
+    try:
+        np_, nb, ncol = c_int64(), c_int64(), c_int()
+        ctx.check(lib.b200gp_mg_geometry(mg, byref(np_), byref(nb), byref(ncol)))
+        np_, nb, ncol = np_.value, nb.value, ncol.value
+        assert nb == 512 and ncol == 3 and np_ - 2 * nb == last
+        for J in range(ncol):
+            r0, r1 = multigpu.my_rows(np_, J * nb, 1, 0)
+            ctx.check(lib.b200gp_mg_update_rows(mg, J, r0, r1))
+            ctx.check(lib.b200gp_mg_panel_factor(mg, J, r0, r1))
+            ctx.check(lib.b200gp_mg_panel_finish(mg, J))
+        lp = c_double()
+        ctx.check(lib.b200gp_mg_finish(mg, byref(lp)))
+    finally:
+        lib.b200gp_mg_free(mg)
+    want = multigpu.log_probability_sharded(k, X, diag, y, slices=7, streaming=False, ctx=ctx)
+    assert lp.value == want, (lp.value, want)
+    lpo = o.GaussianProcess(to_oracle(k), X, diag=0.1).log_probability(y)
+    assert rel(lp.value, lpo) < LOGP_RTOL, (lp.value, lpo)

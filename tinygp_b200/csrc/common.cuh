@@ -66,13 +66,11 @@ struct b200gp_ctx {
     int64_t qsm_chunk = 0;      // points per warp in the QSM-algebra scans (qsm.cu); 0 = chosen per problem size
     int64_t qsm_sequential_redos = 0;   // read-only counter: Riccati scans redone sequentially after the consistency check (qsm.cu run_ric)
     int64_t qs_tree = 1;        // 1: warp-shuffle scan over the chunk composites (fan-in 32; default), 0: thread-sequential fan-in-16 tree
-    int64_t potf2_version = 2;  // 1: column-at-a-time diagonal-block kernel, 2: rank-8 blocked with register tiles
     int64_t qs_kernel = 1;      // quasiseparable factorisation: 1 = layout-specialised kernels (qs_fast.cuh) when the model's block
                                 // layout is compiled in, 0 = always the generic J x J kernels of qs_core.cuh
     int64_t qs_occupancy = 1;   // structured quasisep kernels: 1 = register-capped variants (16 / 12 resident warps per SM), 0 = natural
     int64_t build_fast = 2;     // kernel-matrix build: 2 = + compile-time single-leaf kernels (coef * one stationary leaf, <= 3-D),
                                 // 1 = sum-of-products normal form when the program has one, 0 = interpreter
-    int64_t panel_fused = 0;    // 1: one launch per 128-column step of the panel factorisation (potf2 + trtri + solve)
     int64_t oz_splitk = 1024;   // int8 update (default launch shape): > 0 = split K over idle SM pairs, value = fixed cost of a tile in K
                                 // columns for the policy (ozaki.cu choose_splitk); 0 = one K range per tile
     int64_t mg_splitk = 0;       // sharded path: 0 (default) = one K range per tile: bit-identical results for every rank count;
@@ -86,9 +84,6 @@ struct b200gp_ctx {
     int64_t oz_lookahead = 0;   // overlap the fp64 panel factorisation with the int8 update on a second stream
     cudaStream_t stream2 = nullptr;
     int64_t build_ahead = 0;    // 1: generate block column J+1 on a side stream under the int8 update of column J
-    int64_t panel_overlap = 2;  // 2 (default): look-ahead, diagonal-block chain on a high-priority stream; 1: rows below the diagonal
-                                // tile on a side stream while potf2 runs; 0: serial
-    cudaStream_t stream3 = nullptr;
     // fused log_probability: residual whose forward substitution dense_factor_ozaki runs panel by panel on a side stream,
     // under the int8 update of the NEXT block column (set by dense_logp_impl, consumed by the factorisation)
     const double* fuse_resid = nullptr;   // n values, host or device
@@ -97,9 +92,7 @@ struct b200gp_ctx {
     double* fuse_x = nullptr;             // np: L^-1 resid once the factorisation has returned
     int64_t solve_overlap = 1;            // option: 1 = hide the forward substitution of log_probability under the factorisation
     cudaStream_t stream_solve = nullptr;
-    int64_t panel_chain = 1;    // look-ahead panel: 1 (default) = right-looking order inside the diagonal block (a shorter chain of
-                                // small kernels per panel), 0 = left-looking (bit-identical to panel_overlap 0 / 1)
-    cudaStream_t stream_hi = nullptr;   // high-priority stream of the look-ahead panel chain (panel_overlap = 2)
+    cudaStream_t stream_hi = nullptr;   // high-priority stream of the panel factorisation's diagonal-block chain
     int64_t oz_prefetch = 0;    // L2 prefetch distance (K-chunks of 128) of the int8 update's TMA producer
     int64_t oz_pairing = 1;    // int8 update: 1 = accumulate two digit groups at once (default: 16 instead of 28 operand-stage loads
                                // per K chunk at 7 planes), 0 = one group per pass, 2 = diagnostic (paired loop order, single groups)

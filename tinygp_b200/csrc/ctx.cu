@@ -183,7 +183,6 @@ int b200gp_destroy(b200gp_ctx* ctx) {
     if (ctx->ev0) cudaEventDestroy(ctx->ev0);
     if (ctx->ev1) cudaEventDestroy(ctx->ev1);
     if (ctx->stream2) cudaStreamDestroy(ctx->stream2);
-    if (ctx->stream3) cudaStreamDestroy(ctx->stream3);
     if (ctx->stream_solve) cudaStreamDestroy(ctx->stream_solve);
     if (ctx->stream_hi) cudaStreamDestroy(ctx->stream_hi);
     if (ctx->own_stream) cudaStreamDestroy(ctx->stream);
@@ -207,16 +206,12 @@ static const struct OptEntry { const char* key; int64_t b200gp_ctx::*field; } kO
     {"build_fast", &b200gp_ctx::build_fast},
     {"qs_kernel", &b200gp_ctx::qs_kernel},
     {"qs_occupancy", &b200gp_ctx::qs_occupancy},
-    {"potf2_version", &b200gp_ctx::potf2_version},
-    {"panel_fused", &b200gp_ctx::panel_fused},
     {"nb_batched", &b200gp_ctx::nb_batched},
     {"ozaki_slices", &b200gp_ctx::oz_slices},
     {"ozaki_prefetch", &b200gp_ctx::oz_prefetch},
     {"ozaki_layout", &b200gp_ctx::oz_layout},
     {"ozaki_pairing", &b200gp_ctx::oz_pairing},
     {"build_ahead", &b200gp_ctx::build_ahead},
-    {"panel_overlap", &b200gp_ctx::panel_overlap},
-    {"panel_chain", &b200gp_ctx::panel_chain},
     {"ozaki_lookahead", &b200gp_ctx::oz_lookahead},
     {"ozaki_cluster", &b200gp_ctx::oz_cluster},
     {"ozaki_min_n", &b200gp_ctx::oz_min_n},
@@ -263,7 +258,6 @@ int b200gp_set_option(b200gp_ctx* ctx, const char* key, int64_t value) {
         validate_option(key, value);
         if (!strcmp(key, "ozaki_pairing")) value = (value == 2) ? 2 : (value ? 1 : 0);
         else if (!strcmp(key, "build_ahead")) value = value ? 1 : 0;
-        else if (!strcmp(key, "panel_overlap")) value = (value == 2) ? 2 : (value ? 1 : 0);
         _ctx->*(o.field) = value;
         return 0;
     }

@@ -535,104 +535,21 @@ static void gemm_nt(b200gp_ctx* ctx, double* C, int64_t ldc, const double* A, in
 }
 
 // =============================================================================================
-// diagonal block: Cholesky of a 128x128 block in shared memory + its triangular inverse.
-// Left-looking column Cholesky; thread (part = tid/128, i = tid%128) owns row i and a quarter of
-// every dot product, so shared-memory accesses are conflict-free (row stride 129 doubles).
+// diagonal block: Cholesky of a 128 x 128 block and its triangular inverse, in shared memory (row stride 129 doubles),
+// one CTA of 512 threads per block (a batched launch: one CTA per problem).
+// The Cholesky is right-looking in steps of 8 columns: every thread that owns a row of the 8-column panel factors the
+// panel's 8 x 8 diagonal block redundantly in registers (no barrier inside) and solves its own row against it; the rank-8
+// update of the trailing triangle then runs on 4 x 4 register tiles (2 FMAs per shared-memory load).  The inverse is
+// built in place 8 columns at a time from the right; thread (part = tid / 128, i = tid % 128) sums a quarter of row i's
+// dot products.  The first bad pivot (NaN or <= 0) goes to *info as global_off + its column + 1 (atomicMin).
 // =============================================================================================
 #define PF_LD 129
 #define PF_THREADS 512
-constexpr int PF_SMEM = (TILE * PF_LD + 4 * TILE + TILE) * (int)sizeof(double);
+constexpr int PF_SMEM = (TILE * PF_LD + TILE * 8 + 4 * TILE * 8) * (int)sizeof(double);
 
-__global__ void __launch_bounds__(PF_THREADS, 1) potf2_trtri_kernel(double* A, int64_t lda, double* linv,
-                                                                    int* info, int global_off, int64_t strideA,
+__global__ void __launch_bounds__(PF_THREADS, 1) potf2_trtri_kernel(double* A, int64_t lda, double* linv, int* info,
+                                                                    int global_off, int64_t strideA,
                                                                     int64_t stride_linv) {
-    extern __shared__ __align__(16) double sm[];
-    A += (int64_t)blockIdx.x * strideA;          // batched launch: one CTA per problem
-    linv += (int64_t)blockIdx.x * stride_linv;
-    info += blockIdx.x;
-    double* S = sm;                     // TILE x PF_LD
-    double* red = sm + TILE * PF_LD;    // 4 x TILE partial sums
-    double* tmp = red + 4 * TILE;       // TILE
-    const int tid = threadIdx.x;
-    const int i = tid & (TILE - 1);
-    const int part = tid >> 7;  // 0..3
-
-    // load lower triangle (coalesced along rows), zero the strict upper part
-    for (int e = tid; e < TILE * TILE; e += PF_THREADS) {
-        const int r = e >> 7, c = e & (TILE - 1);
-        S[r * PF_LD + c] = (c <= r) ? A[(int64_t)r * lda + c] : 0.0;
-    }
-    __syncthreads();
-
-    for (int j = 0; j < TILE; ++j) {
-        // partial dots  sum_{k<j, k = part mod 4} L[i][k] L[j][k]   for rows i >= j
-        double s = 0.0;
-        const double ajj = S[j * PF_LD + j];  // read before anyone overwrites column j
-        const double aij = S[i * PF_LD + j];
-        if (i >= j) {
-            const double* ri = S + i * PF_LD;
-            const double* rj = S + j * PF_LD;
-            for (int k = part; k < j; k += 4) s += ri[k] * rj[k];
-        }
-        red[part * TILE + i] = s;
-        __syncthreads();
-        if (part == 0 && i >= j) {
-            const double vj = ajj - (red[j] + red[TILE + j] + red[2 * TILE + j] + red[3 * TILE + j]);
-            if (i == j) {
-                if (!(vj > 0.0)) atomicMin(info, global_off + j + 1);  // NaN or <= 0: first bad pivot
-                S[j * PF_LD + j] = sqrt(vj);
-            } else {
-                const double vi = aij - (red[i] + red[TILE + i] + red[2 * TILE + i] + red[3 * TILE + i]);
-                S[i * PF_LD + j] = vi / sqrt(vj);
-            }
-        }
-        __syncthreads();
-    }
-
-    // write L back (lower triangle only)
-    for (int e = tid; e < TILE * TILE; e += PF_THREADS) {
-        const int r = e >> 7, c = e & (TILE - 1);
-        if (c <= r) A[(int64_t)r * lda + c] = S[r * PF_LD + c];
-    }
-    __syncthreads();
-
-    // in-place inverse of the lower-triangular S (column sweep from the right, LAPACK dtrti2 order):
-    //   inv[j][j] = 1/L[j][j];  inv[i][j] = -inv[j][j] * sum_{k=j+1..i} inv[i][k] L[k][j],  i > j
-    for (int j = TILE - 1; j >= 0; --j) {
-        if (tid < TILE) tmp[tid] = S[tid * PF_LD + j];  // column j of L (rows >= j valid)
-        __syncthreads();
-        const double dj = 1.0 / tmp[j];
-        double s = 0.0;
-        if (i > j) {
-            const double* ri = S + i * PF_LD;
-            for (int k = j + 1 + part; k <= i; k += 4) s += ri[k] * tmp[k];
-        }
-        red[part * TILE + i] = s;
-        __syncthreads();
-        if (part == 0) {
-            if (i == j)
-                S[j * PF_LD + j] = dj;
-            else if (i > j)
-                S[i * PF_LD + j] = -dj * (red[i] + red[TILE + i] + red[2 * TILE + i] + red[3 * TILE + i]);
-        }
-        __syncthreads();
-    }
-    for (int e = tid; e < TILE * TILE; e += PF_THREADS) {
-        const int r = e >> 7, c = e & (TILE - 1);
-        linv[e] = (c <= r) ? S[r * PF_LD + c] : 0.0;
-    }
-}
-
-// ---- v2: rank-8 blocked right-looking Cholesky + 8-column blocked inverse, register tiles -------------------
-// v1 does 2 shared-memory loads per FMA (no register reuse) and 2-3 barriers per column.
-// Here every 8-column panel is factored redundantly in registers by the threads that own its rows (no barrier
-// inside), the rank-8 trailing update uses 4x4 register tiles (2 FMA per load) and the inverse is built 8 columns
-// at a time: 32 + 48 barriers instead of 640.
-constexpr int PF2_SMEM = (TILE * PF_LD + TILE * 8 + 4 * TILE * 8) * (int)sizeof(double);
-
-__global__ void __launch_bounds__(PF_THREADS, 1) potf2_trtri_kernel_v2(double* A, int64_t lda, double* linv, int* info,
-                                                                       int global_off, int64_t strideA,
-                                                                       int64_t stride_linv) {
     extern __shared__ __align__(16) double sm[];
     A += (int64_t)blockIdx.x * strideA;
     linv += (int64_t)blockIdx.x * stride_linv;
@@ -830,101 +747,35 @@ static void potf2(b200gp_ctx* ctx, double* A, int64_t lda, double* linv, int* in
         CUDA_CHECK(cudaFuncSetAttribute(potf2_trtri_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PF_SMEM));
         attr = true;
     }
-    if (ctx->potf2_version == 1) {
-        potf2_trtri_kernel<<<batch, PF_THREADS, PF_SMEM, ctx->stream>>>(A, lda, linv, info, global_off, strideA, stride_linv);
-    } else {
-        static bool attr2 = false;
-        if (!attr2) {
-            CUDA_CHECK(cudaFuncSetAttribute(potf2_trtri_kernel_v2, cudaFuncAttributeMaxDynamicSharedMemorySize, PF2_SMEM));
-            attr2 = true;
-        }
-        potf2_trtri_kernel_v2<<<batch, PF_THREADS, PF2_SMEM, ctx->stream>>>(A, lda, linv, info, global_off, strideA,
-                                                                          stride_linv);
-    }
+    potf2_trtri_kernel<<<batch, PF_THREADS, PF_SMEM, ctx->stream>>>(A, lda, linv, info, global_off, strideA, stride_linv);
     CUDA_CHECK(cudaGetLastError());
     ctx->launches++;
 }
 
 // =============================================================================================
-// blocked right-looking Cholesky driver (outer panel nb, inner 128-wide left-looking sweep)
+// blocked right-looking Cholesky driver (outer panel nb, 128-wide tile columns inside a panel)
 // =============================================================================================
 __global__ void set_int_kernel(int* p, int v) { *p = v; }
 
-// factor the panel of columns [k0, k0+kb) over all rows >= k0: inner 128-wide left-looking sweep
-static void dense_panel_factor_lookahead(b200gp_dense* s, int64_t k0, int64_t kb, int64_t lo = -1, int64_t hi = -1);
-
-void dense_panel_factor(b200gp_dense* s, int64_t k0, int64_t kb) {
-    b200gp_ctx* ctx = s->ctx;
-    const int64_t np = s->np, ld = s->ld;
-    double* M = s->mat;
-    if (ctx->panel_overlap == 2 && kb > TILE) {
-        dense_panel_factor_lookahead(s, k0, kb);
-        return;
-    }
-    // Option "panel_overlap": potf2 runs on ONE SM (a 128 x 128 Cholesky + inverse is a serial chain) while it only
-    // needs the diagonal tile of the column-block update.  So that update is split: the diagonal tile then potf2 stay
-    // on the main stream, the rows below go to a side stream and are joined before the triangular solve that needs both.
-    const bool overlap = ctx->panel_overlap == 1;
-    cudaStream_t main_stream = ctx->stream;
-    cudaEvent_t e_main = nullptr, e_side = nullptr;
-    if (overlap) {
-        if (!ctx->stream3) CUDA_CHECK(cudaStreamCreateWithFlags(&ctx->stream3, cudaStreamNonBlocking));
-        e_main = ctx->get_event();
-        e_side = ctx->get_event();
-    }
-    for (int64_t j0 = 0; j0 < kb; j0 += TILE) {
-        const int64_t c0 = k0 + j0;
-        const int rows_below = (int)((np - c0) / TILE) - 1;
-        bool side_pending = false;
-        if (j0 > 0) {
-            // column block c0 -= (already factored panel columns) x (rows c0.. of them)^T
-            if (overlap && rows_below > 0) {
-                CUDA_CHECK(cudaEventRecord(e_main, main_stream));            // everything up to the previous solve
-                CUDA_CHECK(cudaStreamWaitEvent(ctx->stream3, e_main, 0));
-                ctx->stream = ctx->stream3;
-                try {
-                    gemm_nt(ctx, M + (c0 + TILE) * ld + c0, ld, M + (c0 + TILE) * ld + k0, ld, M + c0 * ld + k0, ld,
-                            rows_below, 1, (int)j0, -1.0, 1, 0);
-                } catch (...) {
-                    ctx->stream = main_stream;
-                    throw;
-                }
-                ctx->stream = main_stream;
-                CUDA_CHECK(cudaEventRecord(e_side, ctx->stream3));
-                side_pending = true;
-                gemm_nt(ctx, M + c0 * ld + c0, ld, M + c0 * ld + k0, ld, M + c0 * ld + k0, ld, 1, 1, (int)j0, -1.0, 1, 0);
-            } else {
-                gemm_nt(ctx, M + c0 * ld + c0, ld, M + c0 * ld + k0, ld, M + c0 * ld + k0, ld,
-                        (int)((np - c0) / TILE), 1, (int)j0, -1.0, 1, 0);
-            }
-        }
-        potf2(ctx, M + c0 * ld + c0, ld, s->linv + (c0 / TILE) * TILE * TILE, s->info_dev, (int)c0);
-        if (c0 + TILE < np) {
-            if (side_pending) CUDA_CHECK(cudaStreamWaitEvent(main_stream, e_side, 0));
-            // rows below: X = A * inv(L_jj)^T, in place (one tile column, K = 128)
-            gemm_nt(ctx, M + (c0 + TILE) * ld + c0, ld, M + (c0 + TILE) * ld + c0, ld,
-                    s->linv + (c0 / TILE) * TILE * TILE, TILE, (int)((np - c0 - TILE) / TILE), 1, TILE,
-                    1.0, 0, 0);
-        }
-    }
-    if (overlap) {
-        ctx->event_pool.push_back(e_main);
-        ctx->event_pool.push_back(e_side);
-    }
-}
-
-// Look-ahead form of the panel factorisation (option "panel_overlap" = 2): the kb x kb DIAGONAL BLOCK is factored on the
-// main stream -- a chain of small kernels whose length is set by the serial 128 x 128 potf2 steps --
-// while the rows BELOW the block are updated / solved on a side stream, column by column, as soon as the potf2 of that
-// column has produced inv(L_jj).  The wide GEMMs no longer wait for the next potf2 and vice versa; per panel the time
-// becomes ~max(potf2 chain, wide GEMMs) instead of their sum.  Same tiles, same arithmetic: bit-identical results.
-// [lo, hi): the rows below the block this call is responsible for (default: all of them; the sharded path passes its chunk)
-static void dense_panel_factor_lookahead(b200gp_dense* s, int64_t k0, int64_t kb, int64_t lo, int64_t hi) {
+// Panel factorisation of the columns [k0, k0+kb), one 128-wide tile column at a time.  The kb x kb DIAGONAL BLOCK is
+// factored by a chain of small kernels whose length is set by the serial 128 x 128 potf2 steps, while the rows BELOW the
+// block are updated / solved on the caller's stream, tile column by tile column, as soon as the potf2 of that column has
+// produced inv(L_jj).  The wide GEMMs do not wait for the next potf2 and vice versa, so per panel the time is
+// ~max(potf2 chain, wide GEMMs) instead of their sum.
+// Inside the diagonal block the order is right-looking: after a tile column is solved, the remaining (blk - 1) x (blk - 1)
+// lower tiles of the block are updated with K = 128 (up to 28 tiles in parallel) instead of each tile column being updated
+// just before its potf2 with K = j0 (1-7 tiles, a single CTA running the longest K).  The rows below are updated
+// left-looking: tile column c0 of them with K = j0 (all earlier columns of the panel) just before its solve.
+// [r0, r1): the rows below the block this call solves.  The sharded path passes its rank's chunk (every rank factors the
+// diagonal block redundantly); the tiles and their arithmetic do not depend on the range, so the rows a rank produces are
+// bit-identical to the unsharded run.
+void dense_panel_factor_rows(b200gp_dense* s, int64_t k0, int64_t kb, int64_t r0, int64_t r1) {
     b200gp_ctx* ctx = s->ctx;
     const int64_t np = s->np, ld = s->ld;
     double* M = s->mat;
     const int64_t bend = k0 + kb;
-    if (lo < 0) { lo = bend; hi = np; }
+    const int64_t lo = (r0 > bend) ? r0 : bend, hi = (r1 < np) ? r1 : np;
+    if (lo % TILE || hi % TILE) throw GpError("panel_factor_rows: row range must be 128-aligned");
     const int own = (hi > lo) ? (int)((hi - lo) / TILE) : 0;
     cudaStream_t wide = ctx->stream;            // the caller's stream keeps the wide GEMMs (and the ProfTimer events)
     // The chain of small kernels runs on a HIGH-PRIORITY stream: when an SM frees up, the block scheduler then places the
@@ -940,25 +791,19 @@ static void dense_panel_factor_lookahead(b200gp_dense* s, int64_t k0, int64_t kb
     struct Restore { b200gp_ctx* c; cudaStream_t st; ~Restore() { c->stream = st; } } restore{ctx, wide};
     CUDA_CHECK(cudaEventRecord(ev, wide));      // the chain must see the block column as the caller left it
     CUDA_CHECK(cudaStreamWaitEvent(chain, ev, 0));
-    // chain_right (option "panel_chain" = 1): RIGHT-looking order inside the diagonal block -- after the block column is
-    // solved, the remaining (blk - 1) x (blk - 1) lower tiles of the block are updated with K = 128 (up to 28 tiles in
-    // parallel) instead of updating each block column just before its potf2 with K = j0 (1-7 tiles, a single CTA running
-    // the longest K).  Shorter chain per panel, different summation order of the
-    // diagonal block (not bit-identical to the left-looking orders).
-    const bool chain_right = (ctx->panel_chain == 1);
     for (int64_t j0 = 0; j0 < kb; j0 += TILE) {
         const int64_t c0 = k0 + j0;
         const int blk = (int)((bend - c0) / TILE);
         const double* li = s->linv + (c0 / TILE) * TILE * TILE;
         ctx->stream = chain;
-        if (j0 > 0 && !chain_right)
-            gemm_nt(ctx, M + c0 * ld + c0, ld, M + c0 * ld + k0, ld, M + c0 * ld + k0, ld, blk, 1, (int)j0, -1.0, 1, 0);
         potf2(ctx, M + c0 * ld + c0, ld, s->linv + (c0 / TILE) * TILE * TILE, s->info_dev, (int)c0);
         if (own) CUDA_CHECK(cudaEventRecord(ev, chain));            // L[c0 rows, k0..c0) and inv(L_jj) are final here
-        if (blk > 1) gemm_nt(ctx, M + (c0 + TILE) * ld + c0, ld, M + (c0 + TILE) * ld + c0, ld, li, TILE, blk - 1, 1, TILE, 1.0, 0, 0);
-        if (chain_right && blk > 1)      // trailing tiles of the diagonal block: C -= X X^T, X = the block column just solved
+        if (blk > 1) {
+            gemm_nt(ctx, M + (c0 + TILE) * ld + c0, ld, M + (c0 + TILE) * ld + c0, ld, li, TILE, blk - 1, 1, TILE, 1.0, 0, 0);
+            // trailing tiles of the diagonal block: C -= X X^T, X = the tile column just solved
             gemm_nt(ctx, M + (c0 + TILE) * ld + (c0 + TILE), ld, M + (c0 + TILE) * ld + c0, ld, M + (c0 + TILE) * ld + c0, ld,
                     blk - 1, blk - 1, TILE, -1.0, 1, 1);
+        }
         if (own) {
             CUDA_CHECK(cudaStreamWaitEvent(wide, ev, 0));
             ctx->stream = wide;
@@ -972,34 +817,8 @@ static void dense_panel_factor_lookahead(b200gp_dense* s, int64_t k0, int64_t kb
     ctx->event_pool.push_back(ev);
 }
 
-// Row-restricted panel factorisation for the sharded path: the diagonal block [k0, k0+kb) is factored (every rank does
-// this part redundantly) and the triangular solve is applied to the caller's rows [r0, r1) below the block only.  Tile
-// arithmetic is that of dense_panel_factor, so the rows a rank produces are bit-identical to the unsharded run.
-void dense_panel_factor_rows(b200gp_dense* s, int64_t k0, int64_t kb, int64_t r0, int64_t r1) {
-    b200gp_ctx* ctx = s->ctx;
-    const int64_t np = s->np, ld = s->ld;
-    double* M = s->mat;
-    const int64_t bend = k0 + kb;
-    int64_t lo = (r0 > bend) ? r0 : bend, hi = (r1 < np) ? r1 : np;
-    if (lo % TILE || hi % TILE) throw GpError("panel_factor_rows: row range must be 128-aligned");
-    if (ctx->panel_overlap == 2 && kb > TILE) {
-        dense_panel_factor_lookahead(s, k0, kb, lo, (hi > lo) ? hi : lo);
-        return;
-    }
-    const int own = (hi > lo) ? (int)((hi - lo) / TILE) : 0;
-    for (int64_t j0 = 0; j0 < kb; j0 += TILE) {
-        const int64_t c0 = k0 + j0;
-        const int blk = (int)((bend - c0) / TILE);          // block rows c0 .. bend
-        if (j0 > 0) {
-            gemm_nt(ctx, M + c0 * ld + c0, ld, M + c0 * ld + k0, ld, M + c0 * ld + k0, ld, blk, 1, (int)j0, -1.0, 1, 0);
-            if (own) gemm_nt(ctx, M + lo * ld + c0, ld, M + lo * ld + k0, ld, M + c0 * ld + k0, ld, own, 1, (int)j0, -1.0, 1, 0);
-        }
-        potf2(ctx, M + c0 * ld + c0, ld, s->linv + (c0 / TILE) * TILE * TILE, s->info_dev, (int)c0);
-        const double* li = s->linv + (c0 / TILE) * TILE * TILE;
-        if (blk > 1) gemm_nt(ctx, M + (c0 + TILE) * ld + c0, ld, M + (c0 + TILE) * ld + c0, ld, li, TILE, blk - 1, 1, TILE, 1.0, 0, 0);
-        if (own) gemm_nt(ctx, M + lo * ld + c0, ld, M + lo * ld + c0, ld, li, TILE, own, 1, TILE, 1.0, 0, 0);
-    }
-}
+// the whole panel: every row below the diagonal block
+void dense_panel_factor(b200gp_dense* s, int64_t k0, int64_t kb) { dense_panel_factor_rows(s, k0, kb, k0 + kb, s->np); }
 
 // generate K (+ diag, identity pad) for rows [r0, np), columns [c0, c0+ncols) straight into the matrix
 void dense_build_region(b200gp_dense* s, int64_t r0, int64_t c0, int64_t ncols) {

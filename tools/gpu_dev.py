@@ -29,8 +29,6 @@ if os.environ.get("PAIRING"):
     ctx.set_option("ozaki_pairing", int(os.environ["PAIRING"]))
 if os.environ.get("PREFETCH"):
     ctx.set_option("ozaki_prefetch", int(os.environ["PREFETCH"]))
-if os.environ.get("POTF2"):
-    ctx.set_option("potf2_version", int(os.environ["POTF2"]))
 out["fp64_peak"] = [ctx.measure_fp64_peak() for _ in range(1)]
 print("fp64 peak (dmma, dfma) TF/s:", out["fp64_peak"], flush=True)
 
