@@ -308,7 +308,7 @@ void dense_build_rect(b200gp_ctx* ctx, const KProg& prog, const double* X1, int6
 // =============================================================================================
 // K2 core: NT GEMM on the fp64 tensor pipe.   C (op)= alpha * A(MxK) * B(NxK)^T
 // 128x128 CTA tile, 8 warps (2 x 4), warp tile 64 x 32 = 4 x 4 DMMA m16n8k16 atoms (dmma.cuh),
-// BK = 16 doubles (one 128-byte line per row per stage), 4-stage cp.async pipeline.
+// BK = 16 doubles (one 128-byte line per row per stage), 4-stage cp.async pipeline refilled after each stage's MMAs.
 // =============================================================================================
 namespace gemm {
 constexpr int BM = 128, BN = 128, BK = dmma::BK, STAGES = 4, LDS = dmma::LDS, THREADS = 256;
@@ -414,9 +414,6 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_nt_kernel(const __grid_consta
     for (int kc = 0; kc < KT; ++kc) {
         cp_async_wait<STAGES - 2>();
         __syncthreads();
-        const int nk = kc + STAGES - 1;
-        if (nk < KT) load_stage(nk % STAGES, nk);
-        cp_async_commit();
         if (g.beta_mode == 1 && kc == (KT > C_PREFETCH ? KT - C_PREFETCH : 0)) {
             // the C tile (128 rows x 8 lines of 128 B) into L2, so that the epilogue's reads do not wait on HBM
 #pragma unroll
@@ -429,6 +426,11 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_nt_kernel(const __grid_consta
         const double* as = smem + (kc % STAGES) * STAGE_DOUBLES + wm * dmma::WM * LDS;
         const double* bs = smem + (kc % STAGES) * STAGE_DOUBLES + BM * LDS + wn * dmma::WN * LDS;
         dmma::warp_tile_stage(acc, as, bs, lane);
+        // refill the stage every warp finished before this iteration's barrier.  Issued after the stage's MMAs, so that
+        // the copies' address arithmetic overlaps them instead of delaying the first fragment loads after the barrier.
+        const int nk = kc + STAGES - 1;
+        if (nk < KT) load_stage(nk % STAGES, nk);
+        cp_async_commit();
     }
 
     // epilogue: acc[mi][ni][q] is C(row0 + acc_row(mi), col0 + acc_col(ni, q)); q = 0, 1 are adjacent columns
