@@ -203,6 +203,16 @@ int b200gp_dense_log_probability_dev(b200gp_ctx* ctx, const double* prog, int n_
 int b200gp_dense_log_probability_grad(b200gp_ctx* ctx, const double* prog, int n_instr, const double* X, int64_t n,
                                       int ndim, const double* diag, const double* resid, double* logp, double* dprog,
                                       double* dmetric, double* ddiag, double* alpha);
+/* b200gp_dense_log_probability_grad plus the gradient with respect to the coordinates, from the same contraction:
+ *   dX  n x ndim, row-major (host): d logp / d x_i = sum_{j != i} (alpha_i alpha_j - W_ij) grad_1 k(x_i, x_j).
+ * The kernel is stationary, so grad_1 k(x_i, x_j) depends on x_i - x_j only; at coincident points (x_i = x_j, i != j)
+ * it is taken as 0 (the L1 distance and the L2 Exp leaf have no derivative there).  ndim <= B200GP_METRIC_MAX_DIM.
+ * The other outputs are bitwise equal to b200gp_dense_log_probability_grad's.  The per-tile partials of dX add about
+ * n^2 ndim / 16 bytes of device memory (805 MB at n = 65536, ndim = 3).  Non positive-definite input: logp = -inf and
+ * every output, dX included, is NaN. */
+int b200gp_dense_log_probability_grad_x(b200gp_ctx* ctx, const double* prog, int n_instr, const double* X, int64_t n,
+                                        int ndim, const double* diag, const double* resid, double* logp, double* dprog,
+                                        double* dmetric, double* ddiag, double* alpha, double* dX);
 /* batched hyper-parameter grid (BASELINE config 5): nbatch programs of equal length over one X;
  * diag (n) and resid (n) shared.  logp[nbatch]. */
 int b200gp_dense_log_probability_batched(b200gp_ctx* ctx, const double* progs, int n_instr,

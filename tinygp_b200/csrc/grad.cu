@@ -12,10 +12,22 @@
 //    are then reduced per slot in a fixed-shape tree: no floating-point atomics, bitwise reproducible.
 // Extra device memory: O(n) vectors, 128 x np for the transposed diagonal blocks and the block-column operand, and
 // tiles x 16 partial sums.  No second np x np buffer.
+//
+// b200gp_dense_log_probability_grad_x adds the gradient with respect to the coordinates, from the same epilogue:
+//   d logp / d x_i = sum_{j != i} (alpha_i alpha_j - W_ij) grad_1 k(x_i, x_j)
+// (K_ij and K_ji both depend on x_i, and grad_2 k(x_j, x_i) = grad_1 k(x_i, x_j) for a stationary k).  Each element
+// i > j of a W tile adds w_ij g_ij (g_ij = d k / d delta at delta = x_i - x_j, kgrad.cuh) to row i and subtracts it from
+// row j.  The tile reduces these into per-tile row sums (a warp-shuffle tree per row, then its four warps in order) and
+// column sums (per thread in registers, then the two threads of a column in order) and writes both; dx_reduce_kernel
+// then adds, per point, the row sums of tiles (I, 0..I) and subtracts the column sums of tiles (I..T-1, I) in that
+// order.  No floating-point atomics: bitwise reproducible.  The partials take tiles x 2 x 128 x ndim doubles, about
+// n^2 ndim / 16 bytes: 805 MB at n = 65536, ndim = 3 (2.1 GB at the cap, ndim = 8).  The plain gradient instantiates the
+// tile kernel with DX = false, where none of this is compiled.
 #include "common.cuh"
 #include "dmma.cuh"
 #include "kgrad.cuh"
 #include <limits.h>
+#include <optional>
 
 namespace tg {
 constexpr int BM = 128, BK = dmma::BK, STAGES = 4, LDS = dmma::LDS, THREADS = 256;
@@ -44,6 +56,7 @@ struct Args {
     const double* alphav;   // alpha, padded to np with zeros
     double* wdiag;          // W_ii
     double* partial;        // [tile][KGRAD_MAX_SLOTS]
+    double* dxpart;         // DX: [tile][row sums, column sums][ndim][BM]
 };
 
 __device__ __forceinline__ void cp_async16(void* smem_ptr, const void* gptr) {
@@ -65,7 +78,9 @@ __device__ __forceinline__ const double* block_ptr(const double* base, int64_t l
 }
 
 // 128 x 128 CTA tile, 8 warps (2 x 4) of 64 x 32, the DMMA warp tile of dmma.cuh (mma.sync.m16n8k16.f64), 4-stage
-// cp.async pipeline (the layout of dense.cu's gemm_nt_kernel) over a per-tile K range of 128-blocks
+// cp.async pipeline (the layout of dense.cu's gemm_nt_kernel) over a per-tile K range of 128-blocks.  DX: the CONTRACT
+// epilogue also writes the tile's coordinate-gradient partials.
+template <bool DX>
 __global__ void __launch_bounds__(THREADS, 1) tri_gemm_kernel(const __grid_constant__ Args g) {
     extern __shared__ __align__(16) double smem[];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -157,21 +172,82 @@ __global__ void __launch_bounds__(THREADS, 1) tri_gemm_kernel(const __grid_const
 #pragma unroll
     for (int s = 0; s < KGRAD_MAX_SLOTS; ++s) gs[s] = 0.0;
     const int nd = g.ndim;
-    for (int e = tid; e < BM * BM; e += THREADS) {
-        const int r = e / BM, c = e % BM;
-        const int64_t i = (int64_t)ti * BM + r, j = (int64_t)tj * BM + c;
-        if (i >= g.n || j >= g.n || j > i) continue;
-        const double w = Ws[e];
-        if (i == j) g.wdiag[i] = w;
-        const double wt = ((i == j) ? 1.0 : 2.0) * (g.alphav[i] * g.alphav[j] - w);
-        const double* xa = g.X + i * nd;
-        const double* xb = g.X + j * nd;
-        double dk[KGRAD_MAX_SLOTS];
+    if constexpr (DX) {
+        // thread tid visits column tid % BM and rows tid / BM + 2k: its column sum stays in registers; the 32 lanes of
+        // a warp share the row, reduced by shuffles into rowp[warp % 4][d][row]
+        double* rowp = smem + BM * BM;     // 4 x KGRAD_MAX_DIM x BM doubles: the rest of SMEM_BYTES
+        double gcol[KGRAD_MAX_DIM];
 #pragma unroll
-        for (int s = 0; s < KGRAD_MAX_SLOTS; ++s) dk[s] = 0.0;
-        kgrad_eval(g.P, g.G, nd, [&](int d) { return xa[d] - xb[d]; }, dk);
+        for (int d = 0; d < KGRAD_MAX_DIM; ++d) gcol[d] = 0.0;
+        for (int e = tid; e < BM * BM; e += THREADS) {
+            const int r = e / BM, c = e % BM;
+            const int64_t i = (int64_t)ti * BM + r, j = (int64_t)tj * BM + c;
+            double gx[KGRAD_MAX_DIM];
 #pragma unroll
-        for (int s = 0; s < KGRAD_MAX_SLOTS; ++s) gs[s] += wt * dk[s];
+            for (int d = 0; d < KGRAD_MAX_DIM; ++d) gx[d] = 0.0;
+            if (i < g.n && j < g.n && j <= i) {
+                const double w = Ws[e];
+                if (i == j) g.wdiag[i] = w;
+                const double wt = ((i == j) ? 1.0 : 2.0) * (g.alphav[i] * g.alphav[j] - w);
+                const double* xa = g.X + i * nd;
+                const double* xb = g.X + j * nd;
+                double dk[KGRAD_MAX_SLOTS];
+#pragma unroll
+                for (int s = 0; s < KGRAD_MAX_SLOTS; ++s) dk[s] = 0.0;
+                kgrad_eval<true>(g.P, g.G, nd, [&](int d) { return xa[d] - xb[d]; }, dk, true, gx);
+#pragma unroll
+                for (int s = 0; s < KGRAD_MAX_SLOTS; ++s) gs[s] += wt * dk[s];
+                const double om = (i > j) ? g.alphav[i] * g.alphav[j] - w : 0.0;
+#pragma unroll
+                for (int d = 0; d < KGRAD_MAX_DIM; ++d) gx[d] *= om;
+            }
+#pragma unroll
+            for (int d = 0; d < KGRAD_MAX_DIM; ++d) {
+                if (d < nd) {
+                    gcol[d] += gx[d];
+                    double v = gx[d];
+#pragma unroll
+                    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+                    if (lane == 0) rowp[((warp & 3) * KGRAD_MAX_DIM + d) * BM + r] = v;
+                }
+            }
+        }
+        __syncthreads();
+        double* colp = smem + 2 * THREADS * KGRAD_MAX_SLOTS;   // past the slot reduction's buffer below
+        if (tid >= BM)
+#pragma unroll
+            for (int d = 0; d < KGRAD_MAX_DIM; ++d)
+                if (d < nd) colp[d * BM + tid - BM] = gcol[d];
+        __syncthreads();
+        if (tid < BM) {
+            double* out = g.dxpart + (int64_t)blockIdx.x * 2 * nd * BM;
+#pragma unroll
+            for (int d = 0; d < KGRAD_MAX_DIM; ++d)
+                if (d < nd) {
+                    double rs = rowp[d * BM + tid];
+#pragma unroll
+                    for (int q = 1; q < 4; ++q) rs += rowp[(q * KGRAD_MAX_DIM + d) * BM + tid];
+                    out[d * BM + tid] = rs;
+                    out[(nd + d) * BM + tid] = gcol[d] + colp[d * BM + tid];
+                }
+        }
+    } else {
+        for (int e = tid; e < BM * BM; e += THREADS) {
+            const int r = e / BM, c = e % BM;
+            const int64_t i = (int64_t)ti * BM + r, j = (int64_t)tj * BM + c;
+            if (i >= g.n || j >= g.n || j > i) continue;
+            const double w = Ws[e];
+            if (i == j) g.wdiag[i] = w;
+            const double wt = ((i == j) ? 1.0 : 2.0) * (g.alphav[i] * g.alphav[j] - w);
+            const double* xa = g.X + i * nd;
+            const double* xb = g.X + j * nd;
+            double dk[KGRAD_MAX_SLOTS];
+#pragma unroll
+            for (int s = 0; s < KGRAD_MAX_SLOTS; ++s) dk[s] = 0.0;
+            kgrad_eval(g.P, g.G, nd, [&](int d) { return xa[d] - xb[d]; }, dk);
+#pragma unroll
+            for (int s = 0; s < KGRAD_MAX_SLOTS; ++s) gs[s] += wt * dk[s];
+        }
     }
     __syncthreads();                   // Ws is reused for the block reduction
     double* red = smem;                // THREADS x KGRAD_MAX_SLOTS
@@ -227,30 +303,47 @@ __global__ void mirror_lower_kernel(double* M, int64_t ld) {
     }
 }
 
+// dX[i][d] = sum_{J <= I} row sums of tile (I, J) - sum_{I' >= I} column sums of tile (I', I), I = i / BM, in this order
+__global__ void __launch_bounds__(BM) dx_reduce_kernel(const double* dxpart, int T, int nd, int64_t n, double* dX) {
+    const int I = blockIdx.x, d = blockIdx.y, r = threadIdx.x;
+    const int64_t stride = 2 * (int64_t)nd * BM;
+    double s = 0.0;
+    const double* p = dxpart + ((int64_t)I * (I + 1) / 2) * stride + d * BM + r;
+#pragma unroll 4
+    for (int J = 0; J <= I; ++J) s += p[J * stride];
+#pragma unroll 4
+    for (int I2 = I; I2 < T; ++I2) s -= dxpart[((int64_t)I2 * (I2 + 1) / 2 + I) * stride + (nd + d) * BM + r];
+    const int64_t i = (int64_t)I * BM + r;
+    if (i < n) dX[i * nd + d] = s;
+}
+
 __global__ void finish_diag_kernel(const double* alphav, const double* wdiag, int64_t n, double* ddiag) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) ddiag[i] = 0.5 * (alphav[i] * alphav[i] - wdiag[i]);
 }
 
+template <bool DX = false>
 static void launch(b200gp_ctx* ctx, const Args& g, unsigned nblocks) {
     static bool attr = false;
     if (!attr) {
-        CUDA_CHECK(cudaFuncSetAttribute(tri_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+        CUDA_CHECK(cudaFuncSetAttribute(tri_gemm_kernel<DX>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
         attr = true;
     }
     if (nblocks == 0) return;
-    tri_gemm_kernel<<<nblocks, THREADS, SMEM_BYTES, ctx->stream>>>(g);
+    tri_gemm_kernel<DX><<<nblocks, THREADS, SMEM_BYTES, ctx->stream>>>(g);
     CUDA_CHECK(cudaGetLastError());
     ctx->launches++;
 }
 }  // namespace tg
 
-extern "C" int b200gp_dense_log_probability_grad(b200gp_ctx* ctx, const double* prog, int n_instr, const double* X,
-                                                 int64_t n, int ndim, const double* diag, const double* resid,
-                                                 double* logp, double* dprog, double* dmetric, double* ddiag,
-                                                 double* alpha) {
+// both entry points; dX == nullptr: the plain gradient (tri_gemm_kernel<false>)
+static int dense_log_probability_grad(b200gp_ctx* ctx, const double* prog, int n_instr, const double* X, int64_t n,
+                                      int ndim, const double* diag, const double* resid, double* logp, double* dprog,
+                                      double* dmetric, double* ddiag, double* alpha, double* dX) {
     API_BEGIN(ctx)
     const KProg P = parse_prog(prog, n_instr, ndim);
+    if (dX != nullptr && (ndim < 1 || ndim > KGRAD_MAX_DIM))
+        throw GpError("log_probability_grad_x: coordinate gradients support 1 to 8 input dimensions");
     KGrad G;
     if (!kgrad_prepare(P, G))
         throw GpError("log_probability_grad: the kernel program has more than 16 differentiable parameters, or a leaf "
@@ -283,6 +376,8 @@ extern "C" int b200gp_dense_log_probability_grad(b200gp_ctx* ctx, const double* 
         for (int m = 0; m < P.nmetric; ++m)
             for (int r = 0; r < P.mrows[m]; ++r) dmetric[m * B200GP_METRIC_MAX_DIM + r] = nan;
         for (int64_t i = 0; i < n; ++i) ddiag[i] = alpha[i] = nan;
+        if (dX != nullptr)
+            for (int64_t i = 0; i < n * ndim; ++i) dX[i] = nan;
         return 0;
     }
     *logp = lp;
@@ -318,6 +413,12 @@ extern "C" int b200gp_dense_log_probability_grad(b200gp_ctx* ctx, const double* 
     const int64_t ntiles = (int64_t)T * (T + 1) / 2;
     Scratch part_buf(_ctx, (size_t)ntiles * KGRAD_MAX_SLOTS * 8), wd_buf(_ctx, (size_t)np * 8),
         xd_buf(_ctx, (size_t)n * ndim * 8), g_buf(_ctx, KGRAD_MAX_SLOTS * 8), dd_buf(_ctx, (size_t)n * 8);
+    const bool want_dx = dX != nullptr;
+    std::optional<Scratch> dxp_buf, dx_buf;
+    if (want_dx) {
+        dxp_buf.emplace(_ctx, (size_t)ntiles * 2 * ndim * TILE * 8);
+        dx_buf.emplace(_ctx, (size_t)n * ndim * 8);
+    }
     {
         ProfTimer t(_ctx, &_ctx->prof.contract_ms);
         tg::mirror_lower_kernel<<<dim3((unsigned)(np / 32), (unsigned)(np / 32)), dim3(32, 8), 0, _ctx->stream>>>(M, ld);
@@ -330,7 +431,15 @@ extern "C" int b200gp_dense_log_probability_grad(b200gp_ctx* ctx, const double* 
         g.P = P; g.G = G;
         g.X = xd_buf.f64(); g.ndim = ndim; g.n = n;
         g.alphav = av; g.wdiag = wd_buf.f64(); g.partial = part_buf.f64();
-        tg::launch(_ctx, g, (unsigned)ntiles);
+        if (want_dx) {
+            g.dxpart = dxp_buf->f64();
+            tg::launch<true>(_ctx, g, (unsigned)ntiles);
+            tg::dx_reduce_kernel<<<dim3((unsigned)T, (unsigned)ndim), tg::BM, 0, _ctx->stream>>>(dxp_buf->f64(), T, ndim, n,
+                                                                                           dx_buf->f64());
+            _ctx->launches++;
+        } else {
+            tg::launch(_ctx, g, (unsigned)ntiles);
+        }
         tg::slot_reduce_kernel<<<KGRAD_MAX_SLOTS, 1024, 0, _ctx->stream>>>(part_buf.f64(), ntiles, g_buf.f64());
         tg::finish_diag_kernel<<<(unsigned)((n + 255) / 256), 256, 0, _ctx->stream>>>(av, wd_buf.f64(), n, dd_buf.f64());
         _ctx->launches += 2;
@@ -340,6 +449,7 @@ extern "C" int b200gp_dense_log_probability_grad(b200gp_ctx* ctx, const double* 
     CUDA_CHECK(cudaMemcpyAsync(gh, g_buf.p, sizeof(gh), cudaMemcpyDeviceToHost, _ctx->stream));
     CUDA_CHECK(cudaMemcpyAsync(ddiag, dd_buf.p, (size_t)n * 8, cudaMemcpyDeviceToHost, _ctx->stream));
     CUDA_CHECK(cudaMemcpyAsync(alpha, av, (size_t)n * 8, cudaMemcpyDeviceToHost, _ctx->stream));
+    if (want_dx) CUDA_CHECK(cudaMemcpyAsync(dX, dx_buf->p, (size_t)n * ndim * 8, cudaMemcpyDeviceToHost, _ctx->stream));
     CUDA_CHECK(cudaStreamSynchronize(_ctx->stream));
     const int row0 = nrows - P.n;      // metric definitions come first
     for (int i = 0; i < P.n; ++i) {
@@ -349,4 +459,24 @@ extern "C" int b200gp_dense_log_probability_grad(b200gp_ctx* ctx, const double* 
     for (int m = 0; m < P.nmetric; ++m)
         for (int r = 0; r < P.mrows[m]; ++r) dmetric[m * B200GP_METRIC_MAX_DIM + r] = gh[G.mslot[m] + r];
     API_END
+}
+
+extern "C" int b200gp_dense_log_probability_grad(b200gp_ctx* ctx, const double* prog, int n_instr, const double* X,
+                                                 int64_t n, int ndim, const double* diag, const double* resid,
+                                                 double* logp, double* dprog, double* dmetric, double* ddiag,
+                                                 double* alpha) {
+    return dense_log_probability_grad(ctx, prog, n_instr, X, n, ndim, diag, resid, logp, dprog, dmetric, ddiag, alpha,
+                                      nullptr);
+}
+
+extern "C" int b200gp_dense_log_probability_grad_x(b200gp_ctx* ctx, const double* prog, int n_instr, const double* X,
+                                                   int64_t n, int ndim, const double* diag, const double* resid,
+                                                   double* logp, double* dprog, double* dmetric, double* ddiag,
+                                                   double* alpha, double* dX) {
+    if (dX == nullptr) {
+        if (ctx) ctx->err = "log_probability_grad_x: dX is NULL";
+        return ctx ? 2 : 1;
+    }
+    return dense_log_probability_grad(ctx, prog, n_instr, X, n, ndim, diag, resid, logp, dprog, dmetric, ddiag, alpha,
+                                      dX);
 }

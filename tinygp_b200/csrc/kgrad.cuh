@@ -8,10 +8,21 @@
 //   - one row-scale sensitivity per row r of each metric m: d k / d lambda at lambda = 1 when row r of M_m is scaled by
 //     lambda (what a 0- / 1-D transforms.Linear or transforms.Cholesky needs).
 // Slots are numbered in program order: for each instruction, its p0 then its p1; then the metric rows, metric by metric.
+//
+// kgrad_eval<true> also returns the gradient of k with respect to the coordinate difference delta = x1 - x2 (what
+// b200gp_dense_log_probability_grad_x needs; for a stationary kernel it is grad_1 k(x1, x2) = -grad_2 k(x1, x2)).  A
+// leaf reads its distance on z = M delta (M = I without a transform), so with f' = d leaf / d distance:
+//   L1:  r = |z|_1,   grad = f'(r) M^T sign(z)
+//   L2:  r = |z|_2,   grad = f'(r) M^T z / r
+//   leaves on the squared distance s (ExpSquared, RationalQuadratic):  grad = 2 f'(s) M^T z  (L1: s = r^2, as above)
+// sums and products chain through the leaf adjoints (the normal form's term products, the interpreter's reverse pass).
+// At coincident points (z = 0) the gradient is defined as 0: L1 takes sign(0) = 0, and the L2 leaves that are not
+// smooth there (Exp, whose f'(0) = -1 / scale gives a direction-dependent limit) contribute 0 instead of NaN.
 #pragma once
 #include "kprog.cuh"
 
 #define KGRAD_MAX_SLOTS 16
+#define KGRAD_MAX_DIM B200GP_METRIC_MAX_DIM     // coordinate gradients: at most this many input dimensions
 
 struct KGrad {
     int nslot;
@@ -82,6 +93,8 @@ __host__ __device__ __forceinline__ double kgrad_leaf(const int op, const bool l
     return v;
 }
 
+__host__ __device__ __forceinline__ double kgrad_sign(const double z) { return (z > 0.0) ? 1.0 : ((z < 0.0) ? -1.0 : 0.0); }
+
 // host: slot layout and operand indices of a parsed program; false if it has more than KGRAD_MAX_SLOTS slots or an
 // opcode without derivatives (the closed forms of quasiseparable kernels)
 static inline bool kgrad_prepare(const KProg& P, KGrad& G) {
@@ -134,11 +147,24 @@ static inline bool kgrad_prepare(const KProg& P, KGrad& G) {
 }
 
 // k(x1, x2) and dk[s] = d k / d slot s for s < G.nslot (`diff(d)` = x1_d - x2_d as in kprog_eval).  use_fast = false
-// forces the interpreter on programs that have a normal form (the CPU check compares the two).
-template <typename F>
+// forces the interpreter on programs that have a normal form (the CPU check compares the two).  DX: also
+// gx[d] = d k / d delta_d for d < ndim (ndim <= KGRAD_MAX_DIM) and 0 for the other KGRAD_MAX_DIM entries; dk is
+// computed by the same arithmetic either way.
+template <bool DX = false, typename F>
 __host__ __device__ __forceinline__ double kgrad_eval(const KProg& P, const KGrad& G, int ndim, F diff, double* dk,
-                                                      bool use_fast = true) {
+                                                      bool use_fast = true, double* gx = nullptr) {
     for (int s = 0; s < G.nslot; ++s) dk[s] = 0.0;
+    // gradient of the identity-metric leaves: a1 * sign(delta) + 2 a2 * delta, with a1 / a2 = d k / d l1 / d l2sq
+    auto identity_dx = [&](const double a1, const double a2) {
+#pragma unroll
+        for (int d = 0; d < KGRAD_MAX_DIM; ++d) {
+            gx[d] = 0.0;
+            if (d < ndim) {
+                const double df = diff(d);
+                gx[d] = a1 * kgrad_sign(df) + 2.0 * a2 * df;
+            }
+        }
+    };
     double l1_id = 0.0, l2_id = 0.0;
     for (int d = 0; d < ndim; ++d) {
         const double df = diff(d);
@@ -147,12 +173,10 @@ __host__ __device__ __forceinline__ double kgrad_eval(const KProg& P, const KGra
     }
     if (G.fast && use_fast) {
         const KFast& K = G.F;
-        double v[KFAST_MAX], d0[KFAST_MAX], d1[KFAST_MAX];
-        for (int i = 0; i < K.nleaf; ++i) {
-            double dl1, dl2sq;
-            v[i] = kgrad_leaf(K.op[i], K.l2[i] != 0, K.p0[i], K.p1[i], l1_id, l2_id, d0[i], d1[i], dl1, dl2sq);
-        }
-        double k = 0.0;
+        double v[KFAST_MAX], d0[KFAST_MAX], d1[KFAST_MAX], gl1[KFAST_MAX], gl2[KFAST_MAX];
+        for (int i = 0; i < K.nleaf; ++i)
+            v[i] = kgrad_leaf(K.op[i], K.l2[i] != 0, K.p0[i], K.p1[i], l1_id, l2_id, d0[i], d1[i], gl1[i], gl2[i]);
+        double k = 0.0, a1 = 0.0, a2 = 0.0;
         for (int t = 0; t < K.nterm; ++t) {
             double prod = 1.0;
             for (int i = 0; i < K.nleaf; ++i)
@@ -166,8 +190,13 @@ __host__ __device__ __forceinline__ double kgrad_eval(const KProg& P, const KGra
                     if (j != i && ((K.mask[t] >> j) & 1)) a *= v[j];
                 dk[G.fslot0[i]] += a * d0[i];
                 if (G.fslot1[i] >= 0) dk[G.fslot1[i]] += a * d1[i];
+                if constexpr (DX) {
+                    a1 += a * gl1[i];
+                    a2 += a * gl2[i];
+                }
             }
         }
+        if constexpr (DX) identity_dx(a1, a2);
         return k;
     }
     // interpreter: values forward, adjoints backward over the postfix program
@@ -216,7 +245,17 @@ __host__ __device__ __forceinline__ double kgrad_eval(const KProg& P, const KGra
             if (G.slot1[i] >= 0) dk[G.slot1[i]] *= a;
         }
     }
+    if constexpr (DX) {
+        double a1 = 0.0, a2 = 0.0;     // gl1 = gl2 = 0 on ADD / MUL / CONST
+        for (int i = 0; i < P.n; ++i)
+            if (P.metric[i] == 0) {
+                a1 += adj[i] * gl1[i];
+                a2 += adj[i] * gl2[i];
+            }
+        identity_dx(a1, a2);
+    }
     // row-scale sensitivities: scaling row r of M_m by lambda moves l2sq by 2 z_r^2 and l1 by |z_r| for every leaf on m
+    // (and delta moves z_r by row r of M_m)
     for (int m = 0; m < P.nmetric; ++m) {
         double g1 = 0.0, g2 = 0.0;
         for (int i = 0; i < P.n; ++i)
@@ -229,6 +268,12 @@ __host__ __device__ __forceinline__ double kgrad_eval(const KProg& P, const KGra
             double z = 0.0;
             for (int c = 0; c < ndim; ++c) z += Mm[r * B200GP_METRIC_MAX_DIM + c] * diff(c);
             dk[G.mslot[m] + r] = 2.0 * z * z * g2 + fabs(z) * g1;
+            if constexpr (DX) {
+                const double gz = g1 * kgrad_sign(z) + 2.0 * g2 * z;
+#pragma unroll
+                for (int c = 0; c < KGRAD_MAX_DIM; ++c)
+                    if (c < ndim) gx[c] += Mm[r * B200GP_METRIC_MAX_DIM + c] * gz;
+            }
         }
     }
     return val[P.n - 1];

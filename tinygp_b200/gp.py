@@ -6,7 +6,7 @@ the six ``Solver`` methods exactly where the reference calls them (gp.py:120,124
 
 from __future__ import annotations
 
-__all__ = ["GaussianProcess", "ConditionResult", "LogProbabilityGrad"]
+__all__ = ["GaussianProcess", "ConditionResult", "LogProbabilityGrad", "LogProbabilityGradX"]
 
 import copy
 from typing import Any, NamedTuple
@@ -73,24 +73,35 @@ class GaussianProcess:
             return loglike if np.isfinite(loglike) else -np.inf
         return self._compute_log_prob(self._get_alpha(y))
 
-    def log_probability_and_grad(self, y) -> tuple[float, "LogProbabilityGrad"]:
+    def log_probability_and_grad(self, y, *, wrt_X: bool = False):
         """``log_probability(y)`` and its exact gradient with respect to the kernel parameters, the noise diagonal and
         the mean, from one device call: the factor, L^-1 in place, and the contraction of (alpha alpha^T - K^-1) with
         dK/dtheta evaluated tile by tile (W = K^-1 is never stored).  Needs the dense DirectSolver, a diagonal noise
         model, and a kernel made of stationary leaves, Constant, sums, products and 0- / 1-D transforms.Linear /
         Cholesky and Subspace, with at most 16 differentiable scalars; anything else raises NotImplementedError.  A
-        non positive-definite covariance gives (-inf, NaN gradients).  The solver's own factor is not touched."""
+        non positive-definite covariance gives (-inf, NaN gradients).  The solver's own factor is not touched.
+
+        Returns ``(logp, LogProbabilityGrad)``; with ``wrt_X=True``, ``(logp, LogProbabilityGradX)``, which also holds
+        d logp / d X with the shape of X, from the same device call (at most 8 input dimensions).  Only the kernel's
+        dependence on X is differentiated: a mean *function* of X is not, and ``grad.mean`` (d logp / d mean) is there to
+        chain through it.  At coincident points the kernel's gradient is taken as 0."""
         hook = getattr(self.solver, "log_probability_grad", None)
         if hook is None:
             raise NotImplementedError(f"log_probability_and_grad: no gradients for {type(self.solver).__name__} (only "
                                       "the dense DirectSolver)")
         yv = np.asarray(y, dtype=np.float64)
-        logp, grads, ddiag, alpha = hook(yv if self._zero_mean else yv - self.loc)
+        resid = yv if self._zero_mean else yv - self.loc
+        if wrt_X:
+            logp, grads, ddiag, alpha, dX = hook(resid, wrt_X=True)
+        else:
+            logp, grads, ddiag, alpha = hook(resid)
         if not np.isfinite(logp):
             logp = -np.inf
-        grad = LogProbabilityGrad(kernel=_grad_tree(self.kernel, grads, {}),
-                                  diag=float(np.sum(ddiag)) if self._scalar_diag else ddiag, mean=alpha)
-        return logp, grad
+        fields = dict(kernel=_grad_tree(self.kernel, grads, {}),
+                      diag=float(np.sum(ddiag)) if self._scalar_diag else ddiag, mean=alpha)
+        if wrt_X:
+            return logp, LogProbabilityGradX(**fields, X=dX.reshape(np.shape(self.X)))
+        return logp, LogProbabilityGrad(**fields)
 
     def condition(self, y, X_test=None, *, diag=None, noise: Noise | None = None, include_mean: bool = True,
                   kernel=None) -> "ConditionResult":
@@ -206,6 +217,16 @@ class LogProbabilityGrad(NamedTuple):
     kernel: Any
     diag: Any
     mean: np.ndarray
+
+
+class LogProbabilityGradX(NamedTuple):
+    """``LogProbabilityGrad`` and ``X``: d logp / d X through the kernel, with the shape of the coordinates ((N,) or
+    (N, D)), from ``log_probability_and_grad(y, wrt_X=True)``.  A mean function of X is not differentiated: chain
+    ``mean`` (= d logp / d mean) through it."""
+    kernel: Any
+    diag: Any
+    mean: np.ndarray
+    X: np.ndarray
 
 
 def _grad_fields(node) -> tuple[str, ...]:

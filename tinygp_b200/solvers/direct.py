@@ -17,6 +17,7 @@ from tinygp_b200.solvers.solver import ConditionedCovariance, Solver
 
 
 MAX_GRAD_SLOTS = 16     # differentiable scalars per kernel program (KGRAD_MAX_SLOTS, tinygp_b200/csrc/kgrad.cuh)
+MAX_GRAD_DIM = 8        # input dimensions of gradients with respect to X (KGRAD_MAX_DIM, tinygp_b200/csrc/kgrad.cuh)
 
 
 class DirectSolver(Solver):
@@ -112,11 +113,13 @@ class DirectSolver(Solver):
             return self._ensure(resid=y)
         return float(np.sum(np.square(self.solve_triangular(y))))
 
-    def log_probability_grad(self, resid):
+    def log_probability_grad(self, resid, wrt_X=False):
         """log_probability and its gradient for the residual ``resid = y - mean`` in one device call
         (b200gp_dense_log_probability_grad), with a factor of its own: the solver's factor, built or pending, is left
         as it is.  Returns (logp, grads, d logp / d diag, alpha) where ``grads`` maps id(node) to (node, {field:
-        d logp / d field}) for every kernel node with a differentiable field reached by the program."""
+        d logp / d field}) for every kernel node with a differentiable field reached by the program.  ``wrt_X``: one
+        call of b200gp_dense_log_probability_grad_x instead, and a fifth item, d logp / d X of shape (N, D) (D = 1 for
+        scalar coordinates), for at most MAX_GRAD_DIM input dimensions."""
         if self._x is None:
             what = ("noise.Dense / noise.Banded" if not isinstance(self.noise, Diagonal)
                     else "a precomputed covariance (covariance=) or a kernel without a device program")
@@ -131,13 +134,26 @@ class DirectSolver(Solver):
             raise NotImplementedError(f"log_probability_and_grad: the kernel has {nslot} differentiable scalars (leaf "
                                       f"scales, constants, gamma / alpha, transform rows); at most {MAX_GRAD_SLOTS} are "
                                       "supported")
+        if wrt_X:
+            if x.shape[1] > MAX_GRAD_DIM:
+                raise NotImplementedError(f"log_probability_and_grad(wrt_X=True): the coordinates have {x.shape[1]} "
+                                          f"dimensions; gradients with respect to X support at most {MAX_GRAD_DIM}")
+            xu = np.asarray(self.X, dtype=np.float64)
+            if x.shape != (self._n, 1 if xu.ndim == 1 else xu.shape[1]) or not np.array_equal(x.reshape(xu.shape), xu):
+                # only transforms.Transform(callable) appends columns, and lower_for_grad refuses it
+                raise AssertionError("log_probability_and_grad(wrt_X=True): the device coordinates differ from X")
         logp = c_double()
         dprog = np.zeros_like(prog)
         dmetric = np.zeros((Lowering.MAX_METRICS, Lowering.MAX_DIM))
         ddiag, alpha = np.empty(self._n), np.empty(self._n)
-        self._ctx.check(self._ctx.lib.b200gp_dense_log_probability_grad(
-            self._ctx.handle, _cabi.ptr(prog), prog.shape[0], _cabi.ptr(x), x.shape[0], x.shape[1], _cabi.ptr(self._diag),
-            _cabi.ptr(resid), byref(logp), _cabi.ptr(dprog), _cabi.ptr(dmetric), _cabi.ptr(ddiag), _cabi.ptr(alpha)))
+        args = (self._ctx.handle, _cabi.ptr(prog), prog.shape[0], _cabi.ptr(x), x.shape[0], x.shape[1],
+                _cabi.ptr(self._diag), _cabi.ptr(resid), byref(logp), _cabi.ptr(dprog), _cabi.ptr(dmetric),
+                _cabi.ptr(ddiag), _cabi.ptr(alpha))
+        if wrt_X:
+            dX = np.empty(x.shape)
+            self._ctx.check(self._ctx.lib.b200gp_dense_log_probability_grad_x(*args, _cabi.ptr(dX)))
+        else:
+            self._ctx.check(self._ctx.lib.b200gp_dense_log_probability_grad(*args))
         grads: dict[int, tuple[Any, dict]] = {}
 
         def add(node, field, value, index=None):
@@ -164,6 +180,8 @@ class DirectSolver(Solver):
                     s = float(v) if v.ndim == 0 else float(v[idx])
                     g = 0.0 if s == 0.0 else (R / s if kind == "linear" else -R / s)
                     add(node, field, g, idx)
+        if wrt_X:
+            return logp.value, grads, ddiag, alpha, dX
         return logp.value, grads, ddiag, alpha
 
     def __del__(self):
