@@ -202,3 +202,9 @@ double dense_logdet_half(b200gp_dense* s);
 void dense_solve_vec_dev(b200gp_dense* s, double* y_dev /* np, destroyed */, double* x_dev /* np */,
                          bool transpose);
 double dense_sumsq_dev(b200gp_ctx* ctx, const double* x_dev, int64_t n);
+// C (op)= alpha A B^T on the fp64 tensor pipe, over tiles_m x tiles_n tiles of 128 x 128 (lower: only the tiles of a square
+// C's lower triangle), K a multiple of 16; A's rows start every lda doubles, B's every ldb, both K-contiguous.  beta_mode
+// 0: C = alpha AB, 1: C += alpha AB.  batch > 1: that many problems, strideA / B / C elements apart.
+void gemm_nt(b200gp_ctx* ctx, double* C, int64_t ldc, const double* A, int64_t lda, const double* B, int64_t ldb,
+             int tiles_m, int tiles_n, int K, double alpha, int beta_mode, int lower, int batch = 1, int64_t strideA = 0,
+             int64_t strideB = 0, int64_t strideC = 0);

@@ -307,13 +307,11 @@ void dense_build_rect(b200gp_ctx* ctx, const KProg& prog, const double* X1, int6
 
 // =============================================================================================
 // K2 core: NT GEMM on the fp64 tensor pipe.   C (op)= alpha * A(MxK) * B(NxK)^T
-// 128x128 CTA tile, 8 warps (2 x 4), warp tile 64 x 32 = 4 x 4 DMMA m16n8k16 atoms (dmma.cuh),
-// BK = 16 doubles (one 128-byte line per row per stage), 4-stage cp.async pipeline refilled after each stage's MMAs.
+// The 128 x 128 CTA tile's mainloop is dmma.cuh's cta_tile_nt (DMMA m16n8k16, 4-stage cp.async ring), which grad.cu's
+// tile kernel runs too; this kernel adds the tile schedules and the beta_mode epilogues.
 // =============================================================================================
 namespace gemm {
-constexpr int BM = 128, BN = 128, BK = dmma::BK, STAGES = 4, LDS = dmma::LDS, THREADS = 256;
-constexpr int STAGE_DOUBLES = (BM + BN) * LDS;
-constexpr int SMEM_BYTES = STAGES * STAGE_DOUBLES * (int)sizeof(double);  // 163840
+using dmma::BM; using dmma::BK; using dmma::THREADS; using dmma::SMEM_BYTES;
 constexpr int BAND = 16;  // tile rows per rasterisation band (L2 reuse of the panel operands)
 constexpr int C_PREFETCH = 4;   // stages before the end of K at which a beta_mode 1 tile of C is prefetched into L2
 
@@ -330,14 +328,6 @@ struct Args {
     // batched launch (blockIdx.y = problem): element strides between problems
     int batch; int64_t strideA, strideB, strideC;
 };
-
-__device__ __forceinline__ void cp_async16(void* smem_ptr, const void* gptr) {
-    const unsigned s = (unsigned)__cvta_generic_to_shared(smem_ptr);
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(s), "l"(gptr));
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
 
 // linear CTA index -> lower-triangular tile (ti, tj), banded so that concurrently resident CTAs
 // share 16 A row-panels and a handful of B row-panels (both stay in L2).
@@ -382,60 +372,29 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_nt_kernel(const __grid_consta
     }
     const int64_t bz = blockIdx.y;
     const double* Ag = g.A + bz * g.strideA + (int64_t)ti * BM * g.lda;
-    const double* Bg = g.B + bz * g.strideB + (int64_t)tj * BN * g.ldb;
-
-    // each thread copies 4 x 16 B of A and 4 x 16 B of B per stage
-    const int lrow = tid >> 3;        // 0..31  (+32 per i)
-    const int lc16 = (tid & 7) * 2;   // double offset of the 16-byte chunk within the 128-byte row
-    auto load_stage = [&](int stage, int kc) {
-        double* as = smem + stage * STAGE_DOUBLES;
-        double* bs = as + BM * LDS;
-        const int64_t koff = (int64_t)kc * BK + lc16;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const int r = lrow + i * 32;
-            cp_async16(as + r * LDS + lc16, Ag + (int64_t)r * g.lda + koff);
-            cp_async16(bs + r * LDS + lc16, Bg + (int64_t)r * g.ldb + koff);
-        }
-    };
+    const double* Bg = g.B + bz * g.strideB + (int64_t)tj * BM * g.ldb;
 
     double acc[8][4][2];
-#pragma unroll
-    for (int mi = 0; mi < 8; ++mi)
-#pragma unroll
-        for (int ni = 0; ni < 4; ++ni) acc[mi][ni][0] = acc[mi][ni][1] = 0.0;
-
     const int KT = g.K / BK;
+    dmma::cta_tile_nt(
+        acc, smem, KT,
+        [&](int kc) { return dmma::Operands{Ag, g.lda, Bg, g.ldb, (int64_t)kc * BK}; },
+        [&](int kc) {
+            if (g.beta_mode == 1 && kc == (KT > C_PREFETCH ? KT - C_PREFETCH : 0)) {
+                // the C tile (128 rows x 8 lines of 128 B) into L2, so that the epilogue's reads do not wait on HBM
 #pragma unroll
-    for (int s = 0; s < STAGES - 1; ++s) {
-        if (s < KT) load_stage(s, s);
-        cp_async_commit();
-    }
-    for (int kc = 0; kc < KT; ++kc) {
-        cp_async_wait<STAGES - 2>();
-        __syncthreads();
-        if (g.beta_mode == 1 && kc == (KT > C_PREFETCH ? KT - C_PREFETCH : 0)) {
-            // the C tile (128 rows x 8 lines of 128 B) into L2, so that the epilogue's reads do not wait on HBM
-#pragma unroll
-            for (int i = 0; i < BM * BN / 16 / THREADS; ++i) {
-                const int line = tid + i * THREADS;
-                const double* p = g.C + bz * g.strideC + ((int64_t)ti * BM + (line >> 3)) * g.ldc + (int64_t)tj * BN + (line & 7) * 16;
-                asm volatile("prefetch.global.L2 [%0];\n" ::"l"(p));
+                for (int i = 0; i < BM * BM / 16 / THREADS; ++i) {
+                    const int line = tid + i * THREADS;
+                    const double* p = g.C + bz * g.strideC + ((int64_t)ti * BM + (line >> 3)) * g.ldc +
+                                      (int64_t)tj * BM + (line & 7) * 16;
+                    asm volatile("prefetch.global.L2 [%0];\n" ::"l"(p));
+                }
             }
-        }
-        const double* as = smem + (kc % STAGES) * STAGE_DOUBLES + wm * dmma::WM * LDS;
-        const double* bs = smem + (kc % STAGES) * STAGE_DOUBLES + BM * LDS + wn * dmma::WN * LDS;
-        dmma::warp_tile_stage(acc, as, bs, lane);
-        // refill the stage every warp finished before this iteration's barrier.  Issued after the stage's MMAs, so that
-        // the copies' address arithmetic overlaps them instead of delaying the first fragment loads after the barrier.
-        const int nk = kc + STAGES - 1;
-        if (nk < KT) load_stage(nk % STAGES, nk);
-        cp_async_commit();
-    }
+        });
 
     // epilogue: acc[mi][ni][q] is C(row0 + acc_row(mi), col0 + acc_col(ni, q)); q = 0, 1 are adjacent columns
     const int64_t crow0 = (int64_t)ti * BM + wm * dmma::WM;
-    const int64_t ccol0 = (int64_t)tj * BN + wn * dmma::WN;
+    const int64_t ccol0 = (int64_t)tj * BM + wn * dmma::WN;
     if (g.beta_mode == 1) {
         // C += alpha AB.  Two accumulator rows' reads are issued before any of their writes: one read-write round trip
         // per element would serialise 32 memory latencies per thread (the compiler cannot move a read of C above a
@@ -524,10 +483,9 @@ static const KProg& empty_prog() {
     return p;
 }
 
-static void gemm_nt(b200gp_ctx* ctx, double* C, int64_t ldc, const double* A, int64_t lda,
-                    const double* B, int64_t ldb, int tiles_m, int tiles_n, int K, double alpha,
-                    int beta_mode, int lower, int batch = 1, int64_t strideA = 0, int64_t strideB = 0,
-                    int64_t strideC = 0) {
+void gemm_nt(b200gp_ctx* ctx, double* C, int64_t ldc, const double* A, int64_t lda, const double* B, int64_t ldb,
+             int tiles_m, int tiles_n, int K, double alpha, int beta_mode, int lower, int batch, int64_t strideA,
+             int64_t strideB, int64_t strideC) {
     gemm::Args g{};
     g.A = A; g.lda = lda; g.B = B; g.ldb = ldb; g.C = C; g.ldc = ldc;
     g.tiles_m = tiles_m; g.tiles_n = tiles_n; g.K = K; g.alpha = alpha;

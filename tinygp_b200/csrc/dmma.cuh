@@ -1,5 +1,7 @@
-// The fp64 tensor-core (DMMA) warp tile shared by every fp64 GEMM mainloop: dense.cu's gemm_nt_kernel (trailing and
-// panel updates) and grad.cu's tri_gemm_kernel (triangular inverse and the W contraction).
+// The fp64 tensor-core (DMMA) mainloop of every fp64 GEMM kernel: the warp tile and the 128 x 128 CTA tile with its
+// cp.async operand ring (cta_tile_nt).  Its callers are dense.cu's gemm_nt_kernel (trailing and panel updates, the
+// gradient's panel products) and grad.cu's tri_gemm_kernel (triangular inverse and the W contraction); each keeps only
+// its tile schedule and its epilogue.
 //
 // Shape: mma.sync.m16n8k16.f64, Hopper's widest fp64 MMA (one DMMA.16x8x16 instruction).  On sm_90 the m16n8 shapes
 // issue at a higher fp64 rate than Ampere's m8n8k4; MEASURED.md records the rates of all four shapes.
@@ -19,6 +21,7 @@
 // The index functions below are __host__ __device__ so that tests/csrc/dmma_hostcheck.cu checks the loads and the
 // accumulator map on the CPU with the same source.
 #pragma once
+#include <stdint.h>
 
 namespace dmma {
 constexpr int MK = 16;                  // K of one mma instruction
@@ -73,6 +76,80 @@ __device__ __forceinline__ void warp_tile_stage(double (&acc)[WM / 8][WN / 8][2]
 #pragma unroll
             for (int ni = 0; ni < AN; ++ni) mma(acc[2 * mi][ni], acc[2 * mi + 1][ni], a, b[ni]);
         }
+    }
+}
+
+// ---- CTA tile: 128 x 128 of C, 8 warps (2 x 4) of warp tiles, 4-stage cp.async ring of BK-deep stages ----
+constexpr int BM = 128, STAGES = 4, THREADS = 256;
+constexpr int STAGE_DOUBLES = 2 * BM * LDS;                                 // A rows, then B rows
+constexpr int SMEM_BYTES = STAGES * STAGE_DOUBLES * (int)sizeof(double);   // 163840
+static_assert(BM == 2 * WM && BM == 4 * WN && THREADS == 8 * 32, "8 warps of 2 x 4 warp tiles cover the CTA tile");
+static_assert(THREADS * 4 * 16 == BM * BK * (int)sizeof(double), "4 rows x 16 B per thread and operand fill a stage");
+
+__device__ __forceinline__ void cp_async16(void* smem_ptr, const void* gptr) {
+    const unsigned s = (unsigned)__cvta_generic_to_shared(smem_ptr);
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(s), "l"(gptr));
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
+
+// K chunk kc of the CTA tile: its A rows start at a, lda doubles apart, its B rows at b, ldb apart; the chunk's BK
+// columns start at column k of both
+struct Operands {
+    const double* a; int64_t lda;
+    const double* b; int64_t ldb;
+    int64_t k;
+};
+
+// acc = (the CTA tile's 128 rows of A) (its 128 rows of B)^T over kchunks chunks of BK, for warp (wm, wn) =
+// (warp / 4, warp % 4) of the block's 8.  operands(kc) -> Operands gives chunk kc's rows; after_barrier(kc) runs once
+// stage kc has landed, before its MMAs.  Each stage is refilled after its MMAs, not right after the barrier: the copies'
+// address arithmetic then overlaps the MMAs instead of delaying every warp's first fragment load (MEASURED.md).  On
+// return every copy has landed (the last STAGES - 1 commit groups are empty), but other warps may still read the last
+// stage: a caller that reuses smem synchronises first.
+template <class ChunkOperands, class AfterBarrier>
+__device__ __forceinline__ void cta_tile_nt(double (&acc)[WM / 8][WN / 8][2], double* smem, int kchunks,
+                                            ChunkOperands operands, AfterBarrier after_barrier) {
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int wm = warp >> 2, wn = warp & 3;
+    // each thread copies 4 rows x 16 B of A and of B per stage
+    const int lrow = tid >> 3;        // 0..31  (+32 per i)
+    const int lc16 = (tid & 7) * 2;   // double offset of the 16-byte chunk within the 128-byte row
+    auto load_stage = [&](int stage, int kc) {
+        const Operands o = operands(kc);
+        const int64_t koff = o.k + lc16;
+        double* as = smem + stage * STAGE_DOUBLES;
+        double* bs = as + BM * LDS;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int r = lrow + i * 32;
+            cp_async16(as + r * LDS + lc16, o.a + (int64_t)r * o.lda + koff);
+            cp_async16(bs + r * LDS + lc16, o.b + (int64_t)r * o.ldb + koff);
+        }
+    };
+
+#pragma unroll
+    for (int mi = 0; mi < WM / 8; ++mi)
+#pragma unroll
+        for (int ni = 0; ni < WN / 8; ++ni) acc[mi][ni][0] = acc[mi][ni][1] = 0.0;
+
+#pragma unroll
+    for (int s = 0; s < STAGES - 1; ++s) {
+        if (s < kchunks) load_stage(s, s);
+        cp_async_commit();
+    }
+    for (int kc = 0; kc < kchunks; ++kc) {
+        cp_async_wait<STAGES - 2>();
+        __syncthreads();
+        after_barrier(kc);
+        const double* as = smem + (kc % STAGES) * STAGE_DOUBLES + wm * WM * LDS;
+        const double* bs = smem + (kc % STAGES) * STAGE_DOUBLES + BM * LDS + wn * WN * LDS;
+        warp_tile_stage(acc, as, bs, lane);
+        // the slot refilled here is the one every warp finished before this iteration's barrier
+        const int nk = kc + STAGES - 1;
+        if (nk < kchunks) load_stage(nk % STAGES, nk);
+        cp_async_commit();
     }
 }
 }  // namespace dmma

@@ -30,16 +30,13 @@
 #include <optional>
 
 namespace tg {
-constexpr int BM = 128, BK = dmma::BK, STAGES = 4, LDS = dmma::LDS, THREADS = 256;
-constexpr int STAGE_DOUBLES = 2 * BM * LDS;
-constexpr int SMEM_BYTES = STAGES * STAGE_DOUBLES * (int)sizeof(double);   // 163840 (>= the 128 x 128 W tile)
-constexpr int CHUNKS = TILE / BK;                                           // K chunks per 128-block
+using dmma::BM; using dmma::BK; using dmma::THREADS; using dmma::SMEM_BYTES;   // SMEM_BYTES >= the 128 x 128 W tile
+constexpr int CHUNKS = TILE / BK;                                               // K chunks per 128-block
 
-// Tile schedules:
-//  PANEL    (inverse, step a): C(0, tj) for tj = j+1 .. T-1, one K block (0)
-//  TRMM     (inverse, step b): C(ti, 0) for ti = T-1 .. j+1 (longest K range first), K blocks j+1 .. ti
-//  CONTRACT (W tiles):          C(ti, tj) for ti >= tj, ti ascending (longest K range first), K blocks ti .. T-1
-enum { PANEL = 0, TRMM = 1, CONTRACT = 2 };
+// Tile schedules (A's row block ti, B's row block tj):
+//  TRMM     (inverse): C(ti, 0) for ti = T-1 .. j+1 (longest K range first), K blocks j+1 .. ti
+//  CONTRACT (W tiles): C(ti, tj) for ti >= tj, ti ascending (longest K range first), K blocks ti .. T-1
+enum { TRMM, CONTRACT };
 
 struct Args {
     const double* A; int64_t lda;
@@ -49,7 +46,6 @@ struct Args {
     const double* diagA; const double* diagB;
     double* C; int64_t ldc;
     int mode, j, T;
-    double alpha;
     // CONTRACT epilogue
     KProg P; KGrad G;
     const double* X; int ndim; int64_t n;
@@ -58,14 +54,6 @@ struct Args {
     double* partial;        // [tile][KGRAD_MAX_SLOTS]
     double* dxpart;         // DX: [tile][row sums, column sums][ndim][BM]
 };
-
-__device__ __forceinline__ void cp_async16(void* smem_ptr, const void* gptr) {
-    const unsigned s = (unsigned)__cvta_generic_to_shared(smem_ptr);
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(s), "l"(gptr));
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
 
 __device__ __forceinline__ const double* block_ptr(const double* base, int64_t ld, const double* diag, int rowblk, int kblk,
                                                    int64_t& ldo) {
@@ -77,18 +65,15 @@ __device__ __forceinline__ const double* block_ptr(const double* base, int64_t l
     return base + (int64_t)rowblk * TILE * ld + (int64_t)kblk * TILE;
 }
 
-// 128 x 128 CTA tile, 8 warps (2 x 4) of 64 x 32, the DMMA warp tile of dmma.cuh (mma.sync.m16n8k16.f64), 4-stage
-// cp.async pipeline (the layout of dense.cu's gemm_nt_kernel) over a per-tile K range of 128-blocks.  DX: the CONTRACT
-// epilogue also writes the tile's coordinate-gradient partials.
+// The 128 x 128 CTA tile of dmma.cuh's cta_tile_nt over a per-tile K range of 128-blocks, A's and B's diagonal blocks
+// substituted.  DX: the CONTRACT epilogue also writes the tile's coordinate-gradient partials.
 template <bool DX>
 __global__ void __launch_bounds__(THREADS, 1) tri_gemm_kernel(const __grid_constant__ Args g) {
     extern __shared__ __align__(16) double smem[];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int wm = warp >> 2, wn = warp & 3;
     int ti, tj, klo, khi;
-    if (g.mode == PANEL) {
-        ti = 0; tj = g.j + 1 + (int)blockIdx.x; klo = khi = 0;
-    } else if (g.mode == TRMM) {
+    if (g.mode == TRMM) {
         ti = g.T - 1 - (int)blockIdx.x; tj = 0; klo = g.j + 1; khi = ti;
     } else {
         const int b = (int)blockIdx.x;
@@ -98,51 +83,21 @@ __global__ void __launch_bounds__(THREADS, 1) tri_gemm_kernel(const __grid_const
         tj = b - ti * (ti + 1) / 2;
         klo = ti; khi = g.T - 1;
     }
-    const int arow = (g.mode == TRMM || g.mode == CONTRACT) ? ti : 0;
-    const int brow = (g.mode == TRMM) ? 0 : tj;
-
-    const int lrow = tid >> 3, lc16 = (tid & 7) * 2;
-    auto load_stage = [&](int stage, int kc) {     // kc: chunk index from klo * CHUNKS
-        double* as = smem + stage * STAGE_DOUBLES;
-        double* bs = as + BM * LDS;
-        const int kblk = klo + kc / CHUNKS;
-        const int koff = (kc % CHUNKS) * BK + lc16;
-        int64_t la, lb;
-        const double* Ab = block_ptr(g.A, g.lda, g.diagA, arow, kblk, la);
-        const double* Bb = block_ptr(g.B, g.ldb, g.diagB, brow, kblk, lb);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const int r = lrow + i * 32;
-            cp_async16(as + r * LDS + lc16, Ab + (int64_t)r * la + koff);
-            cp_async16(bs + r * LDS + lc16, Bb + (int64_t)r * lb + koff);
-        }
-    };
 
     double acc[8][4][2];
-#pragma unroll
-    for (int mi = 0; mi < 8; ++mi)
-#pragma unroll
-        for (int ni = 0; ni < 4; ++ni) acc[mi][ni][0] = acc[mi][ni][1] = 0.0;
+    dmma::cta_tile_nt(
+        acc, smem, (khi - klo + 1) * CHUNKS,
+        [&](int kc) {
+            const int kblk = klo + kc / CHUNKS, k0 = (kc % CHUNKS) * BK;
+            dmma::Operands o;
+            o.a = block_ptr(g.A, g.lda, g.diagA, ti, kblk, o.lda);
+            o.b = block_ptr(g.B, g.ldb, g.diagB, tj, kblk, o.ldb);
+            o.k = k0;
+            return o;
+        },
+        [](int) {});
 
-    const int KT = (khi - klo + 1) * CHUNKS;
-#pragma unroll
-    for (int s = 0; s < STAGES - 1; ++s) {
-        if (s < KT) load_stage(s, s);
-        cp_async_commit();
-    }
-    for (int kc = 0; kc < KT; ++kc) {
-        cp_async_wait<STAGES - 2>();
-        __syncthreads();
-        const int nk = kc + STAGES - 1;
-        if (nk < KT) load_stage(nk % STAGES, nk);
-        cp_async_commit();
-        const double* as = smem + (kc % STAGES) * STAGE_DOUBLES + wm * dmma::WM * LDS;
-        const double* bs = smem + (kc % STAGES) * STAGE_DOUBLES + BM * LDS + wn * dmma::WN * LDS;
-        dmma::warp_tile_stage(acc, as, bs, lane);
-    }
-    cp_async_wait<0>();
-
-    if (g.mode != CONTRACT) {
+    if (g.mode == TRMM) {
         const int64_t crow0 = (int64_t)ti * BM + wm * dmma::WM;
         const int64_t ccol0 = (int64_t)tj * BM + wn * dmma::WN;
 #pragma unroll
@@ -151,7 +106,7 @@ __global__ void __launch_bounds__(THREADS, 1) tri_gemm_kernel(const __grid_const
 #pragma unroll
             for (int ni = 0; ni < 4; ++ni)
                 *reinterpret_cast<double2*>(crow + ccol0 + dmma::acc_col(lane, ni, 0)) =
-                    make_double2(g.alpha * acc[mi][ni][0], g.alpha * acc[mi][ni][1]);
+                    make_double2(acc[mi][ni][0], acc[mi][ni][1]);
         }
         return;
     }
@@ -395,15 +350,12 @@ static int dense_log_probability_grad(b200gp_ctx* ctx, const double* prog, int n
         // X = L^-1 in place: for j = T-2 .. 0,  X_ij = sum_{k=j+1..i} X_ik (-L_kj X_jj)  for i > j;  X_jj = linv_j
         ProfTimer t(_ctx, &_ctx->prof.trtri_ms);
         for (int j = T - 2; j >= 0; --j) {
-            tg::Args g{};
-            // Pt (128 x np, columns k > j) = -(L_kj X_jj)^T = -X_jj^T L_kj^T
-            g.mode = tg::PANEL; g.j = j; g.T = T; g.alpha = -1.0;
-            g.A = linvT + (int64_t)j * TILE * TILE; g.lda = TILE;
-            g.B = M + (int64_t)j * TILE; g.ldb = ld;
-            g.C = Pt; g.ldc = np;
-            tg::launch(_ctx, g, (unsigned)(T - 1 - j));
+            // Pt (128 x np, column blocks k > j) = -(L_kj X_jj)^T = -X_jj^T L_kj^T
+            gemm_nt(_ctx, Pt + (int64_t)(j + 1) * TILE, np, linvT + (int64_t)j * TILE * TILE, TILE,
+                    M + (int64_t)(j + 1) * TILE * ld + (int64_t)j * TILE, ld, 1, T - 1 - j, TILE, -1.0, 0, 0);
             // block column j below the diagonal <- X_{i, j+1..i} Pt^T (diagonal blocks of X from linv)
-            g.mode = tg::TRMM; g.alpha = 1.0;
+            tg::Args g{};
+            g.mode = tg::TRMM; g.j = j; g.T = T;
             g.A = M; g.lda = ld; g.diagA = s->linv;
             g.B = Pt; g.ldb = np;
             g.C = M + (int64_t)j * TILE; g.ldc = ld;
@@ -425,7 +377,7 @@ static int dense_log_probability_grad(b200gp_ctx* ctx, const double* prog, int n
         _ctx->launches++;
         CUDA_CHECK(cudaMemcpyAsync(xd_buf.p, X, (size_t)n * ndim * 8, cudaMemcpyDefault, _ctx->stream));
         tg::Args g{};
-        g.mode = tg::CONTRACT; g.T = T; g.alpha = 1.0;
+        g.mode = tg::CONTRACT; g.T = T;
         g.A = M; g.lda = ld; g.diagA = linvT;        // rows of U = X^T; U's diagonal blocks are linv^T
         g.B = M; g.ldb = ld; g.diagB = linvT;
         g.P = P; g.G = G;
