@@ -125,6 +125,19 @@ int b200gp_i8_update_test(b200gp_ctx* ctx, const int8_t* planes, int S, int64_t 
  * The kernel variant follows the context options (ozaki_cluster / ozaki_pairing / ozaki_layout / ...). */
 int b200gp_i8_update_bench(b200gp_ctx* ctx, int64_t rows, int64_t cols, int64_t K, int S, int reps,
                            int64_t ldq, int64_t ldc, double* ms_out, unsigned long long* dbg_out);
+/* diagnostics for the gradient's triangular tile kernel (grad.cu): one launch with the arguments and grid that
+ * b200gp_dense_log_probability_grad uses, on host operands; T 128-blocks, np = 128 T, matrices row-major, diagA the T
+ * 128 x 128 blocks that replace A's diagonal blocks.  Used by the kernel-level tests only.
+ * mode 0 (inverse step, 0 <= j <= T-2): A (np x np), B (128 x np), C (np x np, in/out); tile rows ti = j+1..T-1 of
+ *   block column j of C <- sum_{k=j+1..ti} A_ti,k B_k^T, every other element of C is left as it is.
+ * mode 1 (W tiles, 1 <= n <= np, 1 <= ndim <= 8): U = A with diagonal blocks diagA; for ti >= tj, W_ti,tj =
+ *   sum_{k=ti..T-1} U_ti,k U_tj,k^T weighted as in the gradient with the kernel program (prog, n_instr), X (n x ndim)
+ *   and alpha (n); out: wdiag (n), partial (T (T+1) / 2 x 16 per-tile slot partials) and, with dxpart and dX both
+ *   non-NULL (the coordinate-gradient instantiation), dxpart (per tile [row sums, column sums][ndim][128]) and the
+ *   reduced dX (n x ndim).  B and C are unused. */
+int b200gp_grad_tiles_test(b200gp_ctx* ctx, int mode, int T, int j, const double* A, const double* diagA,
+                           const double* B, double* C, const double* prog, int n_instr, const double* X, int64_t n,
+                           int ndim, const double* alpha, double* wdiag, double* partial, double* dxpart, double* dX);
 /* option keys for b200gp_set_option: "nb", "profile", "peak_iters", "trim",
  * "ozaki_slices" (0 = native fp64 DMMA trailing update; 2..8 = int8 digit planes), "ozaki_min_n". */
 

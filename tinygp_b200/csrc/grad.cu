@@ -432,3 +432,86 @@ extern "C" int b200gp_dense_log_probability_grad_x(b200gp_ctx* ctx, const double
     return dense_log_probability_grad(ctx, prog, n_instr, X, n, ndim, diag, resid, logp, dprog, dmetric, ddiag, alpha,
                                       dX);
 }
+
+// ---- diagnostics entry point: one launch of tri_gemm_kernel on host operands, with the Args and grid of
+// dense_log_probability_grad (include/b200gp.h).  Every size is checked before anything is allocated, so that the
+// kernels read and write only the buffers allocated here.
+extern "C" int b200gp_grad_tiles_test(b200gp_ctx* ctx, int mode, int T, int j, const double* A, const double* diagA,
+                                      const double* B, double* C, const double* prog, int n_instr, const double* X,
+                                      int64_t n, int ndim, const double* alpha, double* wdiag, double* partial,
+                                      double* dxpart, double* dX) {
+    API_BEGIN(ctx)
+    if (T < 1 || (int64_t)T * (T + 1) > INT_MAX) throw GpError("grad tiles test: 1 <= T, T (T + 1) <= INT_MAX");
+    if (A == nullptr || diagA == nullptr) throw GpError("grad tiles test: A and diagA are required");
+    const int64_t np = (int64_t)T * TILE;
+    const size_t sq_bytes = (size_t)np * np * 8, blk_bytes = (size_t)T * TILE * TILE * 8;
+    if (mode == tg::TRMM) {
+        if (j < 0 || j > T - 2) throw GpError("grad tiles test: TRMM needs 0 <= j <= T - 2");
+        if (B == nullptr || C == nullptr) throw GpError("grad tiles test: TRMM needs B and C");
+        const size_t b_bytes = (size_t)TILE * np * 8;
+        Scratch a_buf(_ctx, sq_bytes), d_buf(_ctx, blk_bytes), b_buf(_ctx, b_bytes), c_buf(_ctx, sq_bytes);
+        CUDA_CHECK(cudaMemcpyAsync(a_buf.p, A, sq_bytes, cudaMemcpyHostToDevice, _ctx->stream));
+        CUDA_CHECK(cudaMemcpyAsync(d_buf.p, diagA, blk_bytes, cudaMemcpyHostToDevice, _ctx->stream));
+        CUDA_CHECK(cudaMemcpyAsync(b_buf.p, B, b_bytes, cudaMemcpyHostToDevice, _ctx->stream));
+        CUDA_CHECK(cudaMemcpyAsync(c_buf.p, C, sq_bytes, cudaMemcpyHostToDevice, _ctx->stream));
+        tg::Args g{};
+        g.mode = tg::TRMM; g.j = j; g.T = T;
+        g.A = a_buf.f64(); g.lda = np; g.diagA = d_buf.f64();
+        g.B = b_buf.f64(); g.ldb = np;
+        g.C = c_buf.f64() + (int64_t)j * TILE; g.ldc = np;
+        tg::launch(_ctx, g, (unsigned)(T - 1 - j));
+        CUDA_CHECK(cudaMemcpyAsync(C, c_buf.p, sq_bytes, cudaMemcpyDeviceToHost, _ctx->stream));
+        CUDA_CHECK(cudaStreamSynchronize(_ctx->stream));
+        return 0;
+    }
+    if (mode != tg::CONTRACT) throw GpError("grad tiles test: mode is 0 (TRMM) or 1 (CONTRACT)");
+    if (n < 1 || n > np) throw GpError("grad tiles test: CONTRACT needs 1 <= n <= 128 T");
+    if (ndim < 1 || ndim > KGRAD_MAX_DIM) throw GpError("grad tiles test: CONTRACT needs 1 <= ndim <= 8");
+    if (prog == nullptr || X == nullptr || alpha == nullptr || wdiag == nullptr || partial == nullptr)
+        throw GpError("grad tiles test: CONTRACT needs prog, X, alpha, wdiag and partial");
+    if ((dxpart == nullptr) != (dX == nullptr)) throw GpError("grad tiles test: dxpart and dX go together");
+    const KProg P = parse_prog(prog, n_instr, ndim);
+    KGrad G;
+    if (!kgrad_prepare(P, G))
+        throw GpError("grad tiles test: the kernel program has more than 16 differentiable parameters, or a leaf "
+                      "without derivatives");
+    const bool want_dx = dX != nullptr;
+    const int64_t ntiles = (int64_t)T * (T + 1) / 2;
+    const size_t part_bytes = (size_t)ntiles * KGRAD_MAX_SLOTS * 8, dxp_bytes = (size_t)ntiles * 2 * ndim * TILE * 8,
+                 x_bytes = (size_t)n * ndim * 8;
+    Scratch a_buf(_ctx, sq_bytes), d_buf(_ctx, blk_bytes), x_buf(_ctx, x_bytes), al_buf(_ctx, (size_t)np * 8),
+        wd_buf(_ctx, (size_t)np * 8), part_buf(_ctx, part_bytes);
+    std::optional<Scratch> dxp_buf, dx_buf;
+    if (want_dx) {
+        dxp_buf.emplace(_ctx, dxp_bytes);
+        dx_buf.emplace(_ctx, x_bytes);
+    }
+    CUDA_CHECK(cudaMemcpyAsync(a_buf.p, A, sq_bytes, cudaMemcpyHostToDevice, _ctx->stream));
+    CUDA_CHECK(cudaMemcpyAsync(d_buf.p, diagA, blk_bytes, cudaMemcpyHostToDevice, _ctx->stream));
+    CUDA_CHECK(cudaMemcpyAsync(x_buf.p, X, x_bytes, cudaMemcpyHostToDevice, _ctx->stream));
+    CUDA_CHECK(cudaMemsetAsync(al_buf.p, 0, (size_t)np * 8, _ctx->stream));
+    CUDA_CHECK(cudaMemcpyAsync(al_buf.p, alpha, (size_t)n * 8, cudaMemcpyHostToDevice, _ctx->stream));
+    tg::Args g{};
+    g.mode = tg::CONTRACT; g.T = T;
+    g.A = a_buf.f64(); g.lda = np; g.diagA = d_buf.f64();
+    g.B = a_buf.f64(); g.ldb = np; g.diagB = d_buf.f64();
+    g.P = P; g.G = G;
+    g.X = x_buf.f64(); g.ndim = ndim; g.n = n;
+    g.alphav = al_buf.f64(); g.wdiag = wd_buf.f64(); g.partial = part_buf.f64();
+    if (want_dx) {
+        g.dxpart = dxp_buf->f64();
+        tg::launch<true>(_ctx, g, (unsigned)ntiles);
+        tg::dx_reduce_kernel<<<dim3((unsigned)T, (unsigned)ndim), tg::BM, 0, _ctx->stream>>>(dxp_buf->f64(), T, ndim, n,
+                                                                                       dx_buf->f64());
+        CUDA_CHECK(cudaGetLastError());
+        _ctx->launches++;
+        CUDA_CHECK(cudaMemcpyAsync(dxpart, dxp_buf->p, dxp_bytes, cudaMemcpyDeviceToHost, _ctx->stream));
+        CUDA_CHECK(cudaMemcpyAsync(dX, dx_buf->p, x_bytes, cudaMemcpyDeviceToHost, _ctx->stream));
+    } else {
+        tg::launch(_ctx, g, (unsigned)ntiles);
+    }
+    CUDA_CHECK(cudaMemcpyAsync(wdiag, wd_buf.p, (size_t)n * 8, cudaMemcpyDeviceToHost, _ctx->stream));
+    CUDA_CHECK(cudaMemcpyAsync(partial, part_buf.p, part_bytes, cudaMemcpyDeviceToHost, _ctx->stream));
+    CUDA_CHECK(cudaStreamSynchronize(_ctx->stream));
+    API_END
+}
