@@ -138,6 +138,28 @@ int b200gp_i8_update_bench(b200gp_ctx* ctx, int64_t rows, int64_t cols, int64_t 
 int b200gp_grad_tiles_test(b200gp_ctx* ctx, int mode, int T, int j, const double* A, const double* diagA,
                            const double* B, double* C, const double* prog, int n_instr, const double* X, int64_t n,
                            int ndim, const double* alpha, double* wdiag, double* partial, double* dxpart, double* dX);
+/* diagnostics for the fp64 tensor-core GEMM of the dense factorisation (dense.cu gemm_nt_kernel): one launch with
+ * exactly these arguments on device copies of the host buffers A (a_elems doubles), B (b_elems) and C (c_elems, in/out:
+ * the whole buffer comes back).  For problem p < batch and each computed 128 x 128 tile (ti, tj) -- every tj <= ti < tiles_m
+ * with lower != 0 (then tiles_n == tiles_m), else every ti < tiles_m, tj < tiles_n --
+ *   C_p(ti, tj) = G + alpha sum_{k < K} A_p(ti, k) B_p(tj, k)^T   (A_p = A + p strideA, row r at A_p + r lda; B, C alike),
+ * with G = 0 (beta_mode 0), the tile's previous value (1), or the generator (2): k(x_{row0+i}, x_{col0+j}) from the
+ * kernel program (prog, n_instr) on X (n_valid x ndim), plus diag[row0+i] where row0 + i == col0 + j; 1 on that diagonal
+ * and 0 elsewhere once row0 + i or col0 + j >= n_valid.  K is a positive multiple of 128, the row strides and the
+ * problem strides are even.  Every other element of C is left as it is.  Used by the kernel-level tests only. */
+int b200gp_gemm_nt_test(b200gp_ctx* ctx, const double* A, int64_t a_elems, int64_t lda, int64_t strideA,
+                        const double* B, int64_t b_elems, int64_t ldb, int64_t strideB, double* C, int64_t c_elems,
+                        int64_t ldc, int64_t strideC, int batch, int tiles_m, int tiles_n, int K, double alpha,
+                        int beta_mode, int lower, const double* prog, int n_instr, const double* X, int ndim,
+                        const double* diag, int64_t n_valid, int64_t row0, int64_t col0);
+/* diagnostics for the diagonal-block kernel of the dense factorisation (dense.cu potf2_trtri_kernel): one launch on
+ * device copies of A (a_elems doubles, in/out: the whole buffer comes back), which holds `batch` 128 x 128 blocks at
+ * A + p strideA with row stride lda.  Each block's lower triangle is replaced by its Cholesky factor L (the strict upper
+ * triangle is neither read nor written); linv (batch x 128 x 128) receives L^-1 with zeros above the diagonal; info[p]
+ * = global_off + the 1-based column of the block's first pivot that is not > 0 (NaN included), or 0.  Used by the
+ * kernel-level tests only. */
+int b200gp_potf2_test(b200gp_ctx* ctx, double* A, int64_t a_elems, int64_t lda, int64_t strideA, int batch,
+                      int global_off, double* linv, int* info);
 /* option keys for b200gp_set_option: "nb", "profile", "peak_iters", "trim",
  * "ozaki_slices" (0 = native fp64 DMMA trailing update; 2..8 = int8 digit planes), "ozaki_min_n". */
 

@@ -12,16 +12,19 @@ from util import LOGP_RTOL, assert_close, rel, to_oracle
 pytestmark = pytest.mark.gpu
 
 KERNELS = {
-    "expsq": lambda: kernels.ExpSquared(1.5),
-    "exp": lambda: kernels.Exp(0.7),
-    "m32": lambda: kernels.Matern32(1.5),
-    "m32_l2": lambda: kernels.Matern32(1.5, kernels.L2Distance()),
-    "m52": lambda: kernels.Matern52(2.5),
+    # the single-leaf entries: 4 leaves x 2 metrics, each with an amplitude (the compiled single-leaf build's coef)
+    "expsq": lambda: 1.7 * kernels.ExpSquared(1.5),
+    "expsq_l1": lambda: 1.7 * kernels.ExpSquared(1.5, kernels.L1Distance()),
+    "exp": lambda: 1.7 * kernels.Exp(0.7),
+    "exp_l2": lambda: 1.7 * kernels.Exp(0.7, kernels.L2Distance()),
+    "m32": lambda: 1.7 * kernels.Matern32(1.5),
+    "m32_l2": lambda: 1.7 * kernels.Matern32(1.5, kernels.L2Distance()),
+    "m52": lambda: 1.7 * kernels.Matern52(2.5),
+    "m52_l2": lambda: 1.7 * kernels.Matern52(2.5, kernels.L2Distance()),
     "cos": lambda: kernels.Cosine(2.3),
     "ess": lambda: kernels.ExpSineSquared(2.3, gamma=1.3),
     "rq": lambda: kernels.RationalQuadratic(1.2, alpha=1.7),
     "rq_l2": lambda: kernels.RationalQuadratic(1.2, kernels.L2Distance(), alpha=1.7),
-    "expsq_l1": lambda: kernels.ExpSquared(1.5, kernels.L1Distance()),
     "combo": lambda: 1.8 * kernels.ExpSquared(0.9) + kernels.Matern32(3.0) * kernels.Constant(0.4) + 0.1,
     "c3": lambda: 1.5 * kernels.Matern52(2.0) + 0.7 * kernels.RationalQuadratic(1.5, alpha=1.5),
     # BASELINE config 3 with Euclidean metrics (the L1 defaults are not positive definite for D > 1)
@@ -32,20 +35,24 @@ KERNELS = {
 }
 
 
-@pytest.mark.parametrize("build_fast", [1, 0])     # 1: sum-of-products normal form (default), 0: program interpreter
+# 2: single-leaf programs in 1-3 dimensions run the compiled single-leaf build (the default), others the normal form;
+# 1: the sum-of-products normal form; 0: the program interpreter
+@pytest.mark.parametrize("build_fast", [2, 1, 0])
 @pytest.mark.parametrize("name", sorted(KERNELS))
-@pytest.mark.parametrize("ndim", [1, 3])
+@pytest.mark.parametrize("ndim", [1, 2, 3])
 def test_kernel_matrix_parity(name, ndim, build_fast, ctx):
     ctx.set_option("build_fast", build_fast)          # restored by conftest's autouse fixture
     rng = np.random.default_rng(1234 + ndim)
-    X1 = rng.uniform(-3, 3, (137, ndim)) if ndim > 1 else rng.uniform(-3, 3, 137)
-    X2 = rng.uniform(-3, 3, (61, ndim)) if ndim > 1 else rng.uniform(-3, 3, 61)
+    # 300 x 400 and 300 x 300: the build's 32 x 128 blocks include interior ones (all valid, off the diagonal) as well
+    # as boundary and diagonal ones
+    X1 = rng.uniform(-3, 3, (300, ndim)) if ndim > 1 else rng.uniform(-3, 3, 300)
+    X2 = rng.uniform(-3, 3, (400, ndim)) if ndim > 1 else rng.uniform(-3, 3, 400)
     k = KERNELS[name]()
     ko = to_oracle(k)
     np.testing.assert_allclose(k(X1, X2), ko(X1, X2), rtol=1e-13, atol=1e-15)
     np.testing.assert_allclose(k(X1, X1), ko(X1, X1), rtol=1e-13, atol=1e-15)
     np.testing.assert_allclose(k(X1), ko(X1), rtol=1e-15)
-    y = rng.normal(size=61)
+    y = rng.normal(size=400)
     np.testing.assert_allclose(k.matmul(X1, X2, y), ko(X1, X2) @ y, rtol=1e-11, atol=1e-12)
     # the diagonal of a stationary kernel is exact (explicit differences, distance.py:58-59)
     if name not in ("combo", "c3", "c3_l2", "combo_l2"):
@@ -290,4 +297,74 @@ def test_batched_hyperparameter_grid(ctx):
         ctx.handle, _cabi.ptr(p2), p2.shape[1], 2, _cabi.ptr(X2), n2, 2, _cabi.ptr(d2), _cabi.ptr(y2), _cabi.ptr(out4)))
     for k, got in zip(ks2, out4):
         want = o.GaussianProcess(to_oracle(k), X2, diag=0.05).log_probability(y2)
+        assert rel(got, want) < LOGP_RTOL, (got, want)
+
+
+@pytest.mark.parametrize("nb", [128, 512, 1024])      # n = 1100: the last tile is ragged, the last panel short
+@pytest.mark.parametrize("int8", [False, True])
+def test_info_is_the_first_bad_pivot(int8, nb, ctx):
+    """`info` is LAPACK's dpotrf info (the 1-based column of the first pivot that is not > 0) for a pivot planted at
+    the first and last column of a tile, across a panel boundary and at the last column; NaN on the diagonal is
+    reported at its own column.  log_probability is -inf."""
+    ctx.set_option("nb", nb)
+    if int8:
+        ctx.set_option("ozaki_min_n", 0)                # the int8 trailing update at the default 7 digit planes
+    rng = np.random.default_rng(nb)
+    n = 1100
+    X = rng.uniform(0, 8, (n, 3))
+    y = np.sin(X[:, 0])
+    k = 1.3 * kernels.ExpSquared(0.8)
+    K = to_oracle(k)(X, X)
+    for i in (0, 127, 128, 777, n - 1):
+        for planted in (-(1.3 + 10.0), np.nan):
+            diag = np.full(n, 0.1)
+            diag[i] = planted
+            if np.isnan(planted):
+                want = i + 1
+            else:
+                _, want = scipy.linalg.lapack.dpotrf(K + np.diag(diag), lower=1)
+                assert want == i + 1
+            assert solvers.DirectSolver(k, X, noise.Diagonal(diag)).info == want, (i, planted)
+            assert GaussianProcess(k, X, diag=diag).log_probability(y) == -np.inf, (i, planted)
+
+
+@pytest.mark.parametrize("nb", [128, 4096])
+@pytest.mark.parametrize("grid", ["single_leaf", "mixed"])
+def test_batched_values_do_not_depend_on_the_batch(grid, nb, ctx):
+    """each problem's log-likelihood is bitwise the same in the batch, in the reversed batch and alone: a problem reads
+    only its own constants, program and matrices.  The single-leaf grid runs the compiled build with per-problem
+    constants; the mixed grid (two leaves per program, so also alone) the interpreter."""
+    from tinygp_b200 import _cabi
+    ctx.set_option("nb_batched", nb)
+    rng = np.random.default_rng(17)
+    n = 300
+    X = np.ascontiguousarray(rng.uniform(0, 6, (n, 3)))
+    y = np.sin(X[:, 0]) + 0.1 * rng.normal(size=n)
+    diag = np.full(n, 0.1)
+    L2 = kernels.L2Distance()
+    if grid == "single_leaf":
+        ks = [a * kernels.ExpSquared(s) for s, a in ((0.5, 0.3), (1.0, 1.0), (2.0, 4.0), (1.5, 0.7))]
+    else:
+        ks = [1.3 * kernels.ExpSquared(0.8) + 0.4 * kernels.Matern32(1.1, L2),
+              0.9 * kernels.Matern52(1.5, L2) + 0.2 * kernels.Exp(0.9, L2),
+              1.1 * kernels.RationalQuadratic(1.2, L2, alpha=1.7) + 0.3 * kernels.ExpSquared(2.0),
+              0.5 * kernels.Matern32(0.7, L2) + 0.5 * kernels.Matern52(1.9, L2)]
+    progs = np.ascontiguousarray(np.stack([k.program() for k in ks]))
+
+    def batched(p):
+        p = np.ascontiguousarray(p)
+        out = np.empty(p.shape[0])
+        ctx.check(ctx.lib.b200gp_dense_log_probability_batched(
+            ctx.handle, _cabi.ptr(p), p.shape[1], p.shape[0], _cabi.ptr(X), n, 3, _cabi.ptr(diag), _cabi.ptr(y),
+            _cabi.ptr(out)))
+        return out
+
+    ordered = batched(progs)
+    reversed_ = batched(progs[::-1])[::-1]
+    alone = np.array([batched(progs[b:b + 1])[0] for b in range(len(ks))])
+    assert np.all(np.isfinite(ordered))
+    assert np.array_equal(ordered.view(np.uint64), reversed_.view(np.uint64)), (ordered, reversed_)
+    assert np.array_equal(ordered.view(np.uint64), alone.view(np.uint64)), (ordered, alone)
+    for k, got in zip(ks, ordered):
+        want = o.GaussianProcess(to_oracle(k), X, diag=0.1).log_probability(y)
         assert rel(got, want) < LOGP_RTOL, (got, want)

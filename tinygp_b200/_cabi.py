@@ -54,6 +54,9 @@ SIGNATURES = {
     "b200gp_i8_update_test": (c_int, [_V, _D, _I, _L, _L, _D, _D]),
     "b200gp_i8_update_bench": (c_int, [_V, _L, _L, _L, _I, _I, _L, _L, c_double_p, c_void_p]),
     "b200gp_grad_tiles_test": (c_int, [_V, _I, _I, _I, _D, _D, _D, _D, _D, _I, _D, _L, _I, _D, _D, _D, _D, _D]),
+    "b200gp_gemm_nt_test": (c_int, [_V, _D, _L, _L, _L, _D, _L, _L, _L, _D, _L, _L, _L, _I, _I, _I, _I, c_double, _I, _I,
+                                    _D, _I, _D, _I, _D, _L, _L, _L]),
+    "b200gp_potf2_test": (c_int, [_V, _D, _L, _L, _L, _I, _I, _D, _D]),
     "b200gp_kernel_matrix": (c_int, [_V, _D, _I, _D, _L, _D, _L, _I, _D]),
     "b200gp_kernel_diag": (c_int, [_V, _D, _I, _D, _L, _I, _D]),
     "b200gp_kernel_matvec": (c_int, [_V, _D, _I, _D, _L, _D, _L, _I, _D, _D]),

@@ -13,6 +13,7 @@
 #include "common.cuh"
 #include "dmma.cuh"
 #include <limits.h>
+#include <optional>
 
 // =============================================================================================
 // kernel-program evaluation (device)
@@ -1721,5 +1722,92 @@ extern "C" int b200gp_dense_log_probability_batched(b200gp_ctx* ctx, const doubl
     _ctx->release(dd, (size_t)n * 8);
     _ctx->release(dr, (size_t)n * 8);
     _ctx->release(dl, (size_t)nbatch * 8);
+    API_END
+}
+
+// =============================================================================================
+// diagnostics entry points (include/b200gp.h): one launch of the GEMM or of the diagonal-block kernel on device copies
+// of host buffers.  Every size is checked before anything is allocated, so that the kernels read and write only the
+// buffers allocated here; the whole output buffers come back, so that a write outside the intended elements shows.
+// =============================================================================================
+extern "C" int b200gp_gemm_nt_test(b200gp_ctx* ctx, const double* A, int64_t a_elems, int64_t lda, int64_t strideA,
+                                   const double* B, int64_t b_elems, int64_t ldb, int64_t strideB, double* C,
+                                   int64_t c_elems, int64_t ldc, int64_t strideC, int batch, int tiles_m, int tiles_n,
+                                   int K, double alpha, int beta_mode, int lower, const double* prog, int n_instr,
+                                   const double* X, int ndim, const double* diag, int64_t n_valid, int64_t row0,
+                                   int64_t col0) {
+    API_BEGIN(ctx)
+    using gemm::BM;
+    if (A == nullptr || B == nullptr || C == nullptr) throw GpError("gemm test: A, B and C are required");
+    if (batch < 1 || batch > 65535) throw GpError("gemm test: 1 <= batch <= 65535");
+    if (tiles_m < 1 || tiles_n < 1) throw GpError("gemm test: tiles_m, tiles_n >= 1");
+    if (lower && tiles_n != tiles_m) throw GpError("gemm test: the lower schedule needs tiles_n == tiles_m");
+    const int64_t ntiles = lower ? (int64_t)tiles_m * (tiles_m + 1) / 2 : (int64_t)tiles_m * tiles_n;
+    if (ntiles > INT_MAX) throw GpError("gemm test: too many tiles");
+    if (K < BM || K % BM != 0) throw GpError("gemm test: K is a positive multiple of 128");
+    if (beta_mode < 0 || beta_mode > 2) throw GpError("gemm test: beta_mode is 0, 1 or 2");
+    // 16-byte cp.async operand rows and double2 stores of C: even row strides and problem strides
+    if (lda < K || ldb < K || ldc < (int64_t)tiles_n * BM || ((lda | ldb | ldc) & 1))
+        throw GpError("gemm test: lda, ldb >= K, ldc >= 128 tiles_n, all even");
+    if (strideA < 0 || strideB < 0 || strideC < 0 || ((strideA | strideB | strideC) & 1))
+        throw GpError("gemm test: problem strides are even and >= 0");
+    // footprints in double: exact below 2^53, and no int64 overflow for any argument
+    const double rows_a = (double)tiles_m * BM, rows_b = (double)tiles_n * BM, nb1 = batch - 1;
+    if (a_elems > ((int64_t)1 << 50) || b_elems > ((int64_t)1 << 50) || c_elems > ((int64_t)1 << 50))
+        throw GpError("gemm test: buffers of at most 2^50 elements");
+    if (nb1 * strideA + (rows_a - 1) * lda + K > (double)a_elems) throw GpError("gemm test: A is too small");
+    if (nb1 * strideB + (rows_b - 1) * ldb + K > (double)b_elems) throw GpError("gemm test: B is too small");
+    if (nb1 * strideC + (rows_a - 1) * ldc + rows_b > (double)c_elems) throw GpError("gemm test: C is too small");
+    KProg P{};
+    if (beta_mode == 2) {
+        if (prog == nullptr || X == nullptr || diag == nullptr) throw GpError("gemm test: beta_mode 2 needs prog, X, diag");
+        if (ndim < 1 || ndim > MAX_NDIM) throw GpError("gemm test: ndim must be in [1, 16]");
+        if (n_valid < 1 || row0 < 0 || col0 < 0) throw GpError("gemm test: n_valid >= 1, row0, col0 >= 0");
+        P = parse_prog(prog, n_instr, ndim);
+    }
+    Scratch a_buf(_ctx, (size_t)a_elems * 8), b_buf(_ctx, (size_t)b_elems * 8), c_buf(_ctx, (size_t)c_elems * 8);
+    std::optional<Scratch> x_buf, d_buf;
+    CUDA_CHECK(cudaMemcpyAsync(a_buf.p, A, (size_t)a_elems * 8, cudaMemcpyHostToDevice, _ctx->stream));
+    CUDA_CHECK(cudaMemcpyAsync(b_buf.p, B, (size_t)b_elems * 8, cudaMemcpyHostToDevice, _ctx->stream));
+    CUDA_CHECK(cudaMemcpyAsync(c_buf.p, C, (size_t)c_elems * 8, cudaMemcpyHostToDevice, _ctx->stream));
+    gemm::Args g{};
+    g.A = a_buf.f64(); g.lda = lda; g.B = b_buf.f64(); g.ldb = ldb; g.C = c_buf.f64(); g.ldc = ldc;
+    g.tiles_m = tiles_m; g.tiles_n = tiles_n; g.K = K; g.alpha = alpha; g.beta_mode = beta_mode; g.lower = lower;
+    g.batch = batch; g.strideA = strideA; g.strideB = strideB; g.strideC = strideC;
+    if (beta_mode == 2) {
+        x_buf.emplace(_ctx, (size_t)n_valid * ndim * 8);
+        d_buf.emplace(_ctx, (size_t)n_valid * 8);
+        CUDA_CHECK(cudaMemcpyAsync(x_buf->p, X, (size_t)n_valid * ndim * 8, cudaMemcpyHostToDevice, _ctx->stream));
+        CUDA_CHECK(cudaMemcpyAsync(d_buf->p, diag, (size_t)n_valid * 8, cudaMemcpyHostToDevice, _ctx->stream));
+        g.X = x_buf->f64(); g.diag = d_buf->f64(); g.ndim = ndim; g.n_valid = n_valid; g.row0 = row0; g.col0 = col0;
+    }
+    gemm::launch(_ctx, (beta_mode == 2) ? P : empty_prog(), g);
+    CUDA_CHECK(cudaMemcpyAsync(C, c_buf.p, (size_t)c_elems * 8, cudaMemcpyDeviceToHost, _ctx->stream));
+    CUDA_CHECK(cudaStreamSynchronize(_ctx->stream));
+    API_END
+}
+
+extern "C" int b200gp_potf2_test(b200gp_ctx* ctx, double* A, int64_t a_elems, int64_t lda, int64_t strideA, int batch,
+                                 int global_off, double* linv, int* info) {
+    API_BEGIN(ctx)
+    if (A == nullptr || linv == nullptr || info == nullptr) throw GpError("potf2 test: A, linv and info are required");
+    if (batch < 1 || batch > 65535) throw GpError("potf2 test: 1 <= batch <= 65535");
+    if (lda < TILE || strideA < 0) throw GpError("potf2 test: lda >= 128, strideA >= 0");
+    if (global_off < 0 || global_off > INT_MAX - TILE) throw GpError("potf2 test: 0 <= global_off <= INT_MAX - 128");
+    if (a_elems > ((int64_t)1 << 50) || (double)(batch - 1) * strideA + (double)(TILE - 1) * lda + TILE > (double)a_elems)
+        throw GpError("potf2 test: A is too small");
+    const size_t linv_bytes = (size_t)batch * TILE * TILE * 8;
+    Scratch a_buf(_ctx, (size_t)a_elems * 8), l_buf(_ctx, linv_bytes), i_buf(_ctx, (size_t)batch * sizeof(int));
+    CUDA_CHECK(cudaMemcpyAsync(a_buf.p, A, (size_t)a_elems * 8, cudaMemcpyHostToDevice, _ctx->stream));
+    fill_int_kernel<<<nblocks(batch, 256), 256, 0, _ctx->stream>>>((int*)i_buf.p, INT_MAX, batch);
+    CUDA_CHECK(cudaGetLastError());
+    _ctx->launches++;
+    potf2(_ctx, a_buf.f64(), lda, l_buf.f64(), (int*)i_buf.p, global_off, batch, strideA, (int64_t)TILE * TILE);
+    CUDA_CHECK(cudaMemcpyAsync(A, a_buf.p, (size_t)a_elems * 8, cudaMemcpyDeviceToHost, _ctx->stream));
+    CUDA_CHECK(cudaMemcpyAsync(linv, l_buf.p, linv_bytes, cudaMemcpyDeviceToHost, _ctx->stream));
+    CUDA_CHECK(cudaMemcpyAsync(info, i_buf.p, (size_t)batch * sizeof(int), cudaMemcpyDeviceToHost, _ctx->stream));
+    CUDA_CHECK(cudaStreamSynchronize(_ctx->stream));
+    for (int b = 0; b < batch; ++b)
+        if (info[b] == INT_MAX) info[b] = 0;
     API_END
 }
