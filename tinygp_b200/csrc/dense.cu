@@ -308,13 +308,13 @@ void dense_build_rect(b200gp_ctx* ctx, const KProg& prog, const double* X1, int6
 
 // =============================================================================================
 // K2 core: NT GEMM on the fp64 tensor pipe.   C (op)= alpha * A(MxK) * B(NxK)^T
-// The 128 x 128 CTA tile's mainloop is dmma.cuh's cta_tile_nt (DMMA m16n8k16, 4-stage cp.async ring), which grad.cu's
+// The 128 x 128 CTA tile's mainloop is dmma.cuh's cta_tile_nt (DMMA m16n8k16, 3-slot cp.async ring), which grad.cu's
 // tile kernel runs too; this kernel adds the tile schedules and the beta_mode epilogues.
 // =============================================================================================
 namespace gemm {
-using dmma::BM; using dmma::BK; using dmma::THREADS; using dmma::SMEM_BYTES;
+using dmma::BM; using dmma::SK; using dmma::THREADS; using dmma::SMEM_BYTES;
 constexpr int BAND = 16;  // tile rows per rasterisation band (L2 reuse of the panel operands)
-constexpr int C_PREFETCH = 4;   // stages before the end of K at which a beta_mode 1 tile of C is prefetched into L2
+constexpr int C_PREFETCH = 2;   // stages (64 of K) before the end of K at which a beta_mode 1 tile of C is prefetched into L2
 
 struct Args {
     const double* A; int64_t lda;
@@ -376,10 +376,10 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_nt_kernel(const __grid_consta
     const double* Bg = g.B + bz * g.strideB + (int64_t)tj * BM * g.ldb;
 
     double acc[8][4][2];
-    const int KT = g.K / BK;
+    const int KT = g.K / SK;
     dmma::cta_tile_nt(
         acc, smem, KT,
-        [&](int kc) { return dmma::Operands{Ag, g.lda, Bg, g.ldb, (int64_t)kc * BK}; },
+        [&](int kc) { return dmma::Operands{Ag, g.lda, Bg, g.ldb, (int64_t)kc * SK}; },
         [&](int kc) {
             if (g.beta_mode == 1 && kc == (KT > C_PREFETCH ? KT - C_PREFETCH : 0)) {
                 // the C tile (128 rows x 8 lines of 128 B) into L2, so that the epilogue's reads do not wait on HBM

@@ -6,9 +6,10 @@
 // Shape: mma.sync.m16n8k16.f64, Hopper's widest fp64 MMA (one DMMA.16x8x16 instruction).  On sm_90 the m16n8 shapes
 // issue at a higher fp64 rate than Ampere's m8n8k4; MEASURED.md records the rates of all four shapes.
 //
-// Operands come from one shared-memory pipeline stage: BK = 16 doubles of K per row, rows K-contiguous (both operands
-// of an NT product, C = A B^T), row stride LDS = 20 doubles.  The padding 16 -> 20 makes the fragment loads of a
-// half-warp (rows g = 0..3, k offsets t = 0..3) hit 16 distinct 8-byte bank pairs (row stride 40 words = 8 mod 32).
+// Operands come from one shared-memory pipeline stage: SK = 32 doubles of K per row, rows K-contiguous (both operands
+// of an NT product, C = A B^T), row stride LDS = 36 doubles.  The warp tile steps through a stage BK = 16 of K at a time.
+// The padding 32 -> 36 makes the fragment loads of a half-warp (rows g = 0..3, k offsets t = 0..3) hit 16 distinct
+// 8-byte bank pairs (row stride 72 words = 8 mod 32).
 //
 // A warp owns a WM x WN = 64 x 32 tile of C: 4 x 4 atoms of 16 x 8.  Its accumulators are kept as acc[8][4][2]:
 // acc[m8][ni][q] is C(8 m8 + g, 8 ni + 2 t + q) of the warp tile (acc_row / acc_col), which is what the epilogues
@@ -25,11 +26,11 @@
 
 namespace dmma {
 constexpr int MK = 16;                  // K of one mma instruction
-constexpr int BK = 16, LDS = 20;        // stage depth and padded row stride (doubles)
+constexpr int BK = 16, LDS = 36;        // K step of the warp tile and padded row stride of a stage (doubles)
 constexpr int WM = 64, WN = 32;         // warp tile
 constexpr int AM = WM / 16, AN = WN / 8;
 constexpr int AREG = MK / 2, BREG = MK / 4;
-static_assert(BK % MK == 0, "a stage holds whole mma K steps");
+static_assert(BK % MK == 0, "a warp-tile K step holds whole mma K steps");
 
 __host__ __device__ constexpr int a_row(int lane, int i) { return (lane >> 2) + 8 * (i & 1); }
 __host__ __device__ constexpr int a_k(int lane, int i) { return (lane & 3) + 4 * (i >> 1); }
@@ -61,7 +62,7 @@ __device__ __forceinline__ void mma(double (&lo)[2], double (&hi)[2], const doub
           "d"(b[0]), "d"(b[1]), "d"(b[2]), "d"(b[3]));
 }
 
-// acc += (the warp's 64 rows of A) (its 32 rows of B)^T over one stage of BK
+// acc += (the warp's 64 rows of A) (its 32 rows of B)^T over BK of K
 __device__ __forceinline__ void warp_tile_stage(double (&acc)[WM / 8][WN / 8][2], const double* as, const double* bs,
                                                 int lane) {
 #pragma unroll
@@ -79,22 +80,44 @@ __device__ __forceinline__ void warp_tile_stage(double (&acc)[WM / 8][WN / 8][2]
     }
 }
 
-// ---- CTA tile: 128 x 128 of C, 8 warps (2 x 4) of warp tiles, 4-stage cp.async ring of BK-deep stages ----
-constexpr int BM = 128, STAGES = 4, THREADS = 256;
+// ---- CTA tile: 128 x 128 of C, 8 warps (2 x 4) of warp tiles, 3-slot cp.async ring of SK-deep stages ----
+// Each slot has a full and an empty mbarrier (after the ring, outside the memory a caller reuses).  A warp waits only for
+// the stage it computes on and releases it when its MMAs are done, so there is no CTA barrier in the mainloop: the two
+// warps of an SM sub-partition drift apart and the DMMAs of one overlap the fragment loads of the other.
+constexpr int BM = 128, SK = 32, STAGES = 3, THREADS = 256;
 constexpr int STAGE_DOUBLES = 2 * BM * LDS;                                 // A rows, then B rows
-constexpr int SMEM_BYTES = STAGES * STAGE_DOUBLES * (int)sizeof(double);   // 163840
+constexpr int RING_BYTES = STAGES * STAGE_DOUBLES * (int)sizeof(double);   // 221184
+constexpr int SMEM_BYTES = RING_BYTES + 2 * STAGES * (int)sizeof(uint64_t);
 static_assert(BM == 2 * WM && BM == 4 * WN && THREADS == 8 * 32, "8 warps of 2 x 4 warp tiles cover the CTA tile");
-static_assert(THREADS * 4 * 16 == BM * BK * (int)sizeof(double), "4 rows x 16 B per thread and operand fill a stage");
+static_assert(SK % BK == 0 && SK <= LDS, "a stage holds whole warp-tile K steps");
+static_assert(THREADS * 8 * 16 == BM * SK * (int)sizeof(double), "8 rows x 16 B per thread and operand fill a stage");
 
 __device__ __forceinline__ void cp_async16(void* smem_ptr, const void* gptr) {
     const unsigned s = (unsigned)__cvta_generic_to_shared(smem_ptr);
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(s), "l"(gptr));
 }
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
+__device__ __forceinline__ unsigned bar_addr(uint64_t* bar) { return (unsigned)__cvta_generic_to_shared(bar); }
+__device__ __forceinline__ void mbar_init(uint64_t* bar, unsigned count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(bar_addr(bar)), "r"(count) : "memory");
+}
+// one arrival once every cp.async this thread has issued so far has landed
+__device__ __forceinline__ void mbar_arrive_cp_async(uint64_t* bar) {
+    asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];\n" ::"r"(bar_addr(bar)) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(bar_addr(bar)) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, unsigned parity) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n"
+        "WAIT:\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+        "@!p bra WAIT;\n\t}\n" ::"r"(bar_addr(bar)),
+        "r"(parity)
+        : "memory");
+}
 
-// K chunk kc of the CTA tile: its A rows start at a, lda doubles apart, its B rows at b, ldb apart; the chunk's BK
+// K chunk kc of the CTA tile: its A rows start at a, lda doubles apart, its B rows at b, ldb apart; the chunk's SK
 // columns start at column k of both
 struct Operands {
     const double* a; int64_t lda;
@@ -102,31 +125,40 @@ struct Operands {
     int64_t k;
 };
 
-// acc = (the CTA tile's 128 rows of A) (its 128 rows of B)^T over kchunks chunks of BK, for warp (wm, wn) =
-// (warp / 4, warp % 4) of the block's 8.  operands(kc) -> Operands gives chunk kc's rows; after_barrier(kc) runs once
-// stage kc has landed, before its MMAs.  Each stage is refilled after its MMAs, not right after the barrier: the copies'
-// address arithmetic then overlaps the MMAs instead of delaying every warp's first fragment load (MEASURED.md).  On
-// return every copy has landed (the last STAGES - 1 commit groups are empty), but other warps may still read the last
-// stage: a caller that reuses smem synchronises first.
-template <class ChunkOperands, class AfterBarrier>
+// acc = (the CTA tile's 128 rows of A) (its 128 rows of B)^T over kchunks chunks of SK, for warp (wm, wn) =
+// (warp / 4, warp % 4) of the block's 8.  operands(kc) -> Operands gives chunk kc's rows; after_wait(kc) runs once
+// stage kc has landed, before the warp's MMAs on it.
+//
+// Ring: chunk kc lives in slot kc % STAGES.  Every thread issues its copies of a chunk and arrives on the slot's full
+// barrier when they land (THREADS arrivals); a warp waits on it before its fragment loads.  After its MMAs on chunk kc a
+// warp arrives on the slot's empty barrier (8 arrivals) and then refills the slot of chunk kc - 1 with chunk
+// kc + STAGES - 1, once every warp has released it.  The refill follows the MMAs, so its address arithmetic overlaps
+// them (MEASURED.md), and a warp blocks there only on a warp a whole stage behind it.
+//
+// On return every copy has landed, but other warps may still read the last stages: a caller that reuses smem
+// synchronises first.
+template <class ChunkOperands, class AfterWait>
 __device__ __forceinline__ void cta_tile_nt(double (&acc)[WM / 8][WN / 8][2], double* smem, int kchunks,
-                                            ChunkOperands operands, AfterBarrier after_barrier) {
+                                            ChunkOperands operands, AfterWait after_wait) {
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int wm = warp >> 2, wn = warp & 3;
-    // each thread copies 4 rows x 16 B of A and of B per stage
-    const int lrow = tid >> 3;        // 0..31  (+32 per i)
-    const int lc16 = (tid & 7) * 2;   // double offset of the 16-byte chunk within the 128-byte row
-    auto load_stage = [&](int stage, int kc) {
+    uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<char*>(smem) + RING_BYTES);
+    uint64_t* empty = full + STAGES;
+    // each thread copies 8 rows x 16 B of A and of B per stage
+    const int lrow = tid >> 4;         // 0..15  (+16 per i)
+    const int lc16 = (tid & 15) * 2;   // double offset of the 16-byte chunk within the 256-byte row
+    auto load_stage = [&](int slot, int kc) {
         const Operands o = operands(kc);
         const int64_t koff = o.k + lc16;
-        double* as = smem + stage * STAGE_DOUBLES;
+        double* as = smem + slot * STAGE_DOUBLES;
         double* bs = as + BM * LDS;
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const int r = lrow + i * 32;
+        for (int i = 0; i < 8; ++i) {
+            const int r = lrow + i * 16;
             cp_async16(as + r * LDS + lc16, o.a + (int64_t)r * o.lda + koff);
             cp_async16(bs + r * LDS + lc16, o.b + (int64_t)r * o.ldb + koff);
         }
+        mbar_arrive_cp_async(full + slot);
     };
 
 #pragma unroll
@@ -134,22 +166,39 @@ __device__ __forceinline__ void cta_tile_nt(double (&acc)[WM / 8][WN / 8][2], do
 #pragma unroll
         for (int ni = 0; ni < WN / 8; ++ni) acc[mi][ni][0] = acc[mi][ni][1] = 0.0;
 
+    if (tid == 0)
 #pragma unroll
-    for (int s = 0; s < STAGES - 1; ++s) {
+        for (int s = 0; s < STAGES; ++s) {
+            mbar_init(full + s, THREADS);
+            mbar_init(empty + s, THREADS / 32);
+        }
+    __syncthreads();   // the barriers are initialised before any thread arrives on them
+
+#pragma unroll
+    for (int s = 0; s < STAGES - 1; ++s)
         if (s < kchunks) load_stage(s, s);
-        cp_async_commit();
-    }
+    int slot = 0;
+    unsigned phase = 0;   // parity of chunk kc's use of its slot: (kc / STAGES) & 1
     for (int kc = 0; kc < kchunks; ++kc) {
-        cp_async_wait<STAGES - 2>();
-        __syncthreads();
-        after_barrier(kc);
-        const double* as = smem + (kc % STAGES) * STAGE_DOUBLES + wm * WM * LDS;
-        const double* bs = smem + (kc % STAGES) * STAGE_DOUBLES + BM * LDS + wn * WN * LDS;
-        warp_tile_stage(acc, as, bs, lane);
-        // the slot refilled here is the one every warp finished before this iteration's barrier
+        mbar_wait(full + slot, phase);
+        after_wait(kc);
+        const double* as = smem + slot * STAGE_DOUBLES + wm * WM * LDS;
+        const double* bs = smem + slot * STAGE_DOUBLES + BM * LDS + wn * WN * LDS;
+#pragma unroll
+        for (int k0 = 0; k0 < SK; k0 += BK) warp_tile_stage(acc, as + k0, bs + k0, lane);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty + slot);
         const int nk = kc + STAGES - 1;
-        if (nk < kchunks) load_stage(nk % STAGES, nk);
-        cp_async_commit();
+        if (nk < kchunks) {
+            // chunk kc - 1's slot; its empty phase has chunk kc - 1's parity (none to wait for at kc = 0)
+            const int prev = slot == 0 ? STAGES - 1 : slot - 1;
+            if (kc > 0) mbar_wait(empty + prev, slot == 0 ? phase ^ 1 : phase);
+            load_stage(prev, nk);
+        }
+        if (++slot == STAGES) {
+            slot = 0;
+            phase ^= 1;
+        }
     }
 }
 }  // namespace dmma

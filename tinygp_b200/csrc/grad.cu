@@ -30,8 +30,10 @@
 #include <optional>
 
 namespace tg {
-using dmma::BM; using dmma::BK; using dmma::THREADS; using dmma::SMEM_BYTES;   // SMEM_BYTES >= the 128 x 128 W tile
-constexpr int CHUNKS = TILE / BK;                                               // K chunks per 128-block
+using dmma::BM; using dmma::SK; using dmma::THREADS; using dmma::SMEM_BYTES;   // SMEM_BYTES >= the 128 x 128 W tile
+constexpr int CHUNKS = TILE / SK;                                               // K chunks per 128-block
+// the CONTRACT epilogue's W tile and row sums stay in the operand ring, clear of its mbarriers
+static_assert((BM * BM + 4 * KGRAD_MAX_DIM * BM) * (int)sizeof(double) <= dmma::RING_BYTES, "epilogue fits the ring");
 
 // Tile schedules (A's row block ti, B's row block tj):
 //  TRMM     (inverse): C(ti, 0) for ti = T-1 .. j+1 (longest K range first), K blocks j+1 .. ti
@@ -88,7 +90,7 @@ __global__ void __launch_bounds__(THREADS, 1) tri_gemm_kernel(const __grid_const
     dmma::cta_tile_nt(
         acc, smem, (khi - klo + 1) * CHUNKS,
         [&](int kc) {
-            const int kblk = klo + kc / CHUNKS, k0 = (kc % CHUNKS) * BK;
+            const int kblk = klo + kc / CHUNKS, k0 = (kc % CHUNKS) * SK;
             dmma::Operands o;
             o.a = block_ptr(g.A, g.lda, g.diagA, ti, kblk, o.lda);
             o.b = block_ptr(g.B, g.ldb, g.diagB, tj, kblk, o.ldb);
@@ -130,7 +132,7 @@ __global__ void __launch_bounds__(THREADS, 1) tri_gemm_kernel(const __grid_const
     if constexpr (DX) {
         // thread tid visits column tid % BM and rows tid / BM + 2k: its column sum stays in registers; the 32 lanes of
         // a warp share the row, reduced by shuffles into rowp[warp % 4][d][row]
-        double* rowp = smem + BM * BM;     // 4 x KGRAD_MAX_DIM x BM doubles: the rest of SMEM_BYTES
+        double* rowp = smem + BM * BM;     // 4 x KGRAD_MAX_DIM x BM doubles past the W tile
         double gcol[KGRAD_MAX_DIM];
 #pragma unroll
         for (int d = 0; d < KGRAD_MAX_DIM; ++d) gcol[d] = 0.0;
