@@ -248,6 +248,22 @@ int b200gp_dense_log_probability_grad(b200gp_ctx* ctx, const double* prog, int n
 int b200gp_dense_log_probability_grad_x(b200gp_ctx* ctx, const double* prog, int n_instr, const double* X, int64_t n,
                                         int ndim, const double* diag, const double* resid, double* logp, double* dprog,
                                         double* dmetric, double* ddiag, double* alpha, double* dX);
+/* Expected Fisher information of the Gaussian log-likelihood with respect to the program's differentiable scalars (the
+ * slots of b200gp_dense_log_probability_grad) and, with with_diag = 1, a scalar noise diagonal added to every point
+ * (dK / d diag = I), for a fresh factor that this call builds and frees.  With W = K^-1:
+ *   F_ab = 1/2 tr(W dK_a W dK_b),   computed as 1/2 <dK_a, X^T X dK_b X^T X>, X = L^-1.
+ * It does not depend on any data vector.  Outputs (host):
+ *   nslot   S, the number of program slots (at most 16);
+ *   slots   3 x 16 ints, slot s at 3 s: {0, row, col}: entry (row, col) of the program, col 2 = p0, col 3 = p1 (the
+ *           entries dprog holds); or {1, m, r}: row r of metric m + 1 (the entry (m, r) of dmetric);
+ *   fisher  (S + with_diag)^2 doubles, row-major, rows and columns in slot order, the noise diagonal last.  Symmetric
+ *           bit for bit (each pair of entries is the mean of both contractions).
+ * Refused programs are those of the gradient.  Cost: about 4 (S + with_diag) n^3 flops on top of the factor and L^-1.
+ * Peak memory: that of b200gp_dense_log_probability_grad plus one np x np fp64 work buffer (8.6 GB at n = 32768); if it
+ * cannot be allocated the call fails with a message naming its size.  Deterministic: no floating-point atomics.  Non
+ * positive-definite input does not fail: every entry of fisher is NaN. */
+int b200gp_dense_fisher(b200gp_ctx* ctx, const double* prog, int n_instr, const double* X, int64_t n, int ndim,
+                        const double* diag, int with_diag, int* nslot, int* slots, double* fisher);
 /* batched hyper-parameter grid (BASELINE config 5): nbatch programs of equal length over one X;
  * diag (n) and resid (n) shared.  logp[nbatch]. */
 int b200gp_dense_log_probability_batched(b200gp_ctx* ctx, const double* progs, int n_instr,

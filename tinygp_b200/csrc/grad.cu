@@ -23,6 +23,17 @@
 // order.  No floating-point atomics: bitwise reproducible.  The partials take tiles x 2 x 128 x ndim doubles, about
 // n^2 ndim / 16 bytes: 805 MB at n = 65536, ndim = 3 (2.1 GB at the cap, ndim = 8).  The plain gradient instantiates the
 // tile kernel with DX = false, where none of this is compiled.
+//
+// b200gp_dense_fisher: the expected Fisher information F_ab = 1/2 tr(W dK_a W dK_b) = 1/2 <dK_a, C_b>, C_b = X^T X dK_b
+// X^T X, from the same factor and X = L^-1 (steps 1 and 2, then U = X^T mirrored as in step 3).  For each slot b, in one
+// np x np work buffer:
+//   dK_b (dk_build_kernel; the identity for the noise slot)  -> . X^T -> transpose -> . X^T  = X dK_b X^T = E_b
+//   E_b                                                       -> . X   -> transpose -> . X    = X^T E_b X   = C_b
+// Each ". X^T" / ". X" is an in-place product by a triangular factor on the DMMA mainloop (RMUL_XT / RMUL_X): one launch
+// per output column block, descending (ascending), each CTA owning one row block, so a launch writes exactly the column
+// block that no later launch reads.  Then the contraction tiles (FISHER) read the lower tiles of C_b from memory into the
+// CONTRACT epilogue with weight c_ij in place of alpha_i alpha_j - W_ij; the noise slot's entry is 1/2 tr(C_b) from the
+// C_b diagonal the epilogue writes.  Same fixed-shape reductions as the gradient: bitwise reproducible.
 #include "common.cuh"
 #include "dmma.cuh"
 #include "kgrad.cuh"
@@ -38,7 +49,10 @@ static_assert((BM * BM + 4 * KGRAD_MAX_DIM * BM) * (int)sizeof(double) <= dmma::
 // Tile schedules (A's row block ti, B's row block tj):
 //  TRMM     (inverse): C(ti, 0) for ti = T-1 .. j+1 (longest K range first), K blocks j+1 .. ti
 //  CONTRACT (W tiles): C(ti, tj) for ti >= tj, ti ascending (longest K range first), K blocks ti .. T-1
-enum { TRMM, CONTRACT };
+//  RMUL_XT  (C = A X^T in place, B = X with diagB = linv):    C(ti, j) for every ti, K blocks 0 .. j
+//  RMUL_X   (C = A X in place, B = U = X^T with diagB = linvT): C(ti, j) for every ti, K blocks j .. T-1
+//  FISHER   (Fisher contraction): the tiles of CONTRACT, weight tile read from A, no mainloop
+enum { TRMM, CONTRACT, RMUL_XT, RMUL_X, FISHER };
 
 struct Args {
     const double* A; int64_t lda;
@@ -77,6 +91,10 @@ __global__ void __launch_bounds__(THREADS, 1) tri_gemm_kernel(const __grid_const
     int ti, tj, klo, khi;
     if (g.mode == TRMM) {
         ti = g.T - 1 - (int)blockIdx.x; tj = 0; klo = g.j + 1; khi = ti;
+    } else if (g.mode == RMUL_XT || g.mode == RMUL_X) {
+        ti = (int)blockIdx.x; tj = g.j;
+        klo = (g.mode == RMUL_XT) ? 0 : g.j;
+        khi = (g.mode == RMUL_XT) ? g.j : g.T - 1;
     } else {
         const int b = (int)blockIdx.x;
         ti = (int)((sqrt(8.0 * (double)b + 1.0) - 1.0) * 0.5);
@@ -87,19 +105,20 @@ __global__ void __launch_bounds__(THREADS, 1) tri_gemm_kernel(const __grid_const
     }
 
     double acc[8][4][2];
-    dmma::cta_tile_nt(
-        acc, smem, (khi - klo + 1) * CHUNKS,
-        [&](int kc) {
-            const int kblk = klo + kc / CHUNKS, k0 = (kc % CHUNKS) * SK;
-            dmma::Operands o;
-            o.a = block_ptr(g.A, g.lda, g.diagA, ti, kblk, o.lda);
-            o.b = block_ptr(g.B, g.ldb, g.diagB, tj, kblk, o.ldb);
-            o.k = k0;
-            return o;
-        },
-        [](int) {});
+    if (g.mode != FISHER)
+        dmma::cta_tile_nt(
+            acc, smem, (khi - klo + 1) * CHUNKS,
+            [&](int kc) {
+                const int kblk = klo + kc / CHUNKS, k0 = (kc % CHUNKS) * SK;
+                dmma::Operands o;
+                o.a = block_ptr(g.A, g.lda, g.diagA, ti, kblk, o.lda);
+                o.b = block_ptr(g.B, g.ldb, g.diagB, tj, kblk, o.ldb);
+                o.k = k0;
+                return o;
+            },
+            [](int) {});
 
-    if (g.mode == TRMM) {
+    if (g.mode != CONTRACT && g.mode != FISHER) {
         const int64_t crow0 = (int64_t)ti * BM + wm * dmma::WM;
         const int64_t ccol0 = (int64_t)tj * BM + wn * dmma::WN;
 #pragma unroll
@@ -114,16 +133,22 @@ __global__ void __launch_bounds__(THREADS, 1) tri_gemm_kernel(const __grid_const
     }
 
     // ---- CONTRACT epilogue: W tile -> shared memory, then the derivative pass over its elements ----
-    __syncthreads();                   // every warp is done with the pipeline buffers
+    // (FISHER: the tile of C_b from A instead, and the weight c_ij in place of alpha_i alpha_j - W_ij)
     double* Ws = smem;                 // 128 x 128
+    if (g.mode == FISHER) {
+        const double* src = g.A + (int64_t)ti * BM * g.lda + (int64_t)tj * BM;
+        for (int e = tid; e < BM * BM; e += THREADS) Ws[e] = src[(int64_t)(e / BM) * g.lda + e % BM];
+    } else {
+        __syncthreads();               // every warp is done with the pipeline buffers
 #pragma unroll
-    for (int mi = 0; mi < 8; ++mi)
+        for (int mi = 0; mi < 8; ++mi)
 #pragma unroll
-        for (int ni = 0; ni < 4; ++ni) {
-            const int r = wm * dmma::WM + dmma::acc_row(lane, mi), c = wn * dmma::WN + dmma::acc_col(lane, ni, 0);
-            Ws[r * BM + c] = acc[mi][ni][0];
-            Ws[r * BM + c + 1] = acc[mi][ni][1];
-        }
+            for (int ni = 0; ni < 4; ++ni) {
+                const int r = wm * dmma::WM + dmma::acc_row(lane, mi), c = wn * dmma::WN + dmma::acc_col(lane, ni, 0);
+                Ws[r * BM + c] = acc[mi][ni][0];
+                Ws[r * BM + c + 1] = acc[mi][ni][1];
+            }
+    }
     __syncthreads();
     double gs[KGRAD_MAX_SLOTS];
 #pragma unroll
@@ -195,7 +220,7 @@ __global__ void __launch_bounds__(THREADS, 1) tri_gemm_kernel(const __grid_const
             if (i >= g.n || j >= g.n || j > i) continue;
             const double w = Ws[e];
             if (i == j) g.wdiag[i] = w;
-            const double wt = ((i == j) ? 1.0 : 2.0) * (g.alphav[i] * g.alphav[j] - w);
+            const double wt = ((i == j) ? 1.0 : 2.0) * ((g.mode == FISHER) ? w : g.alphav[i] * g.alphav[j] - w);
             const double* xa = g.X + i * nd;
             const double* xb = g.X + j * nd;
             double dk[KGRAD_MAX_SLOTS];
@@ -219,12 +244,13 @@ __global__ void __launch_bounds__(THREADS, 1) tri_gemm_kernel(const __grid_const
     if (tid < KGRAD_MAX_SLOTS) g.partial[(int64_t)blockIdx.x * KGRAD_MAX_SLOTS + tid] = red[tid * THREADS];
 }
 
-// out[s] = 1/2 sum_t partial[t][s]: one block per slot, fixed-shape tree
-__global__ void __launch_bounds__(1024) slot_reduce_kernel(const double* partial, int64_t ntiles, double* out) {
+// out[s] = 1/2 sum_t partial[t * stride + s]: one block per slot, fixed-shape tree
+__global__ void __launch_bounds__(1024) slot_reduce_kernel(const double* partial, int64_t ntiles, int64_t stride,
+                                                           double* out) {
     __shared__ double sh[1024];
     const int s = blockIdx.x;
     double a = 0.0;
-    for (int64_t t = threadIdx.x; t < ntiles; t += 1024) a += partial[t * KGRAD_MAX_SLOTS + s];
+    for (int64_t t = threadIdx.x; t < ntiles; t += 1024) a += partial[t * stride + s];
     sh[threadIdx.x] = a;
     __syncthreads();
     for (int o = 512; o > 0; o >>= 1) {
@@ -279,6 +305,30 @@ __global__ void finish_diag_kernel(const double* alphav, const double* wdiag, in
     if (i < n) ddiag[i] = 0.5 * (alphav[i] * alphav[i] - wdiag[i]);
 }
 
+// D (np x np) = dK / d slot (kgrad_element): 32 x 8 threads per 32 x 32 tile, 4 rows each
+__global__ void __launch_bounds__(256) dk_build_kernel(const KProg P, const KGrad G, const double* X, int ndim, int64_t n,
+                                                       int64_t np, int slot, double* D) {
+    const int64_t j = (int64_t)blockIdx.x * 32 + threadIdx.x;
+    for (int64_t i = (int64_t)blockIdx.y * 32 + threadIdx.y; i < (int64_t)blockIdx.y * 32 + 32; i += 8)
+        D[i * np + j] = kgrad_element(P, G, ndim, X, n, i, j, slot);
+}
+
+// M (np x np) <- M^T in place: the block at (by, bx), bx <= by, swaps with its mirror (32 x 32 tiles)
+__global__ void transpose_inplace_kernel(double* M, int64_t ld) {
+    __shared__ double a[32][33], b[32][33];
+    const int64_t bi = blockIdx.y, bj = blockIdx.x;
+    if (bj > bi) return;
+    for (int y = threadIdx.y; y < 32; y += 8) {
+        a[y][threadIdx.x] = M[(bi * 32 + y) * ld + bj * 32 + threadIdx.x];
+        b[y][threadIdx.x] = M[(bj * 32 + y) * ld + bi * 32 + threadIdx.x];
+    }
+    __syncthreads();
+    for (int y = threadIdx.y; y < 32; y += 8) {
+        M[(bj * 32 + y) * ld + bi * 32 + threadIdx.x] = a[threadIdx.x][y];
+        M[(bi * 32 + y) * ld + bj * 32 + threadIdx.x] = b[threadIdx.x][y];
+    }
+}
+
 template <bool DX = false>
 static void launch(b200gp_ctx* ctx, const Args& g, unsigned nblocks) {
     static bool attr = false;
@@ -292,6 +342,32 @@ static void launch(b200gp_ctx* ctx, const Args& g, unsigned nblocks) {
     ctx->launches++;
 }
 }  // namespace tg
+
+// step 2: X = L^-1 in place in the lower block triangle of s->mat (its diagonal blocks stay in s->linv); linvT <- the
+// diagonal blocks transposed (T x 128 x 128)
+static void invert_factor(b200gp_ctx* _ctx, b200gp_dense* s, double* linvT) {
+    const int64_t np = s->np, ld = s->np;
+    const int T = (int)(np / TILE);
+    double* const M = s->mat;
+    Scratch pt_buf(_ctx, (size_t)TILE * np * 8);
+    double* const Pt = pt_buf.f64();
+    tg::block_transpose_kernel<<<dim3(TILE / 32, TILE / 32, T), dim3(32, 8), 0, _ctx->stream>>>(s->linv, linvT);
+    _ctx->launches++;
+    // X = L^-1 in place: for j = T-2 .. 0,  X_ij = sum_{k=j+1..i} X_ik (-L_kj X_jj)  for i > j;  X_jj = linv_j
+    ProfTimer t(_ctx, &_ctx->prof.trtri_ms);
+    for (int j = T - 2; j >= 0; --j) {
+        // Pt (128 x np, column blocks k > j) = -(L_kj X_jj)^T = -X_jj^T L_kj^T
+        gemm_nt(_ctx, Pt + (int64_t)(j + 1) * TILE, np, linvT + (int64_t)j * TILE * TILE, TILE,
+                M + (int64_t)(j + 1) * TILE * ld + (int64_t)j * TILE, ld, 1, T - 1 - j, TILE, -1.0, 0, 0);
+        // block column j below the diagonal <- X_{i, j+1..i} Pt^T (diagonal blocks of X from linv)
+        tg::Args g{};
+        g.mode = tg::TRMM; g.j = j; g.T = T;
+        g.A = M; g.lda = ld; g.diagA = s->linv;
+        g.B = Pt; g.ldb = np;
+        g.C = M + (int64_t)j * TILE; g.ldc = ld;
+        tg::launch(_ctx, g, (unsigned)(T - 1 - j));
+    }
+}
 
 // both entry points; dX == nullptr: the plain gradient (tri_gemm_kernel<false>)
 static int dense_log_probability_grad(b200gp_ctx* ctx, const double* prog, int n_instr, const double* X, int64_t n,
@@ -342,28 +418,10 @@ static int dense_log_probability_grad(b200gp_ctx* ctx, const double* prog, int n
     dense_solve_vec_dev(s, yv, av, true);                                  // alpha = L^-T L^-1 r (pad rows: 0)
 
     const size_t blk_bytes = (size_t)T * TILE * TILE * 8;
-    Scratch lt_buf(_ctx, blk_bytes), pt_buf(_ctx, (size_t)TILE * np * 8);
+    Scratch lt_buf(_ctx, blk_bytes);
     double* const linvT = lt_buf.f64();
-    double* const Pt = pt_buf.f64();
     double* const M = s->mat;
-    tg::block_transpose_kernel<<<dim3(TILE / 32, TILE / 32, T), dim3(32, 8), 0, _ctx->stream>>>(s->linv, linvT);
-    _ctx->launches++;
-    {
-        // X = L^-1 in place: for j = T-2 .. 0,  X_ij = sum_{k=j+1..i} X_ik (-L_kj X_jj)  for i > j;  X_jj = linv_j
-        ProfTimer t(_ctx, &_ctx->prof.trtri_ms);
-        for (int j = T - 2; j >= 0; --j) {
-            // Pt (128 x np, column blocks k > j) = -(L_kj X_jj)^T = -X_jj^T L_kj^T
-            gemm_nt(_ctx, Pt + (int64_t)(j + 1) * TILE, np, linvT + (int64_t)j * TILE * TILE, TILE,
-                    M + (int64_t)(j + 1) * TILE * ld + (int64_t)j * TILE, ld, 1, T - 1 - j, TILE, -1.0, 0, 0);
-            // block column j below the diagonal <- X_{i, j+1..i} Pt^T (diagonal blocks of X from linv)
-            tg::Args g{};
-            g.mode = tg::TRMM; g.j = j; g.T = T;
-            g.A = M; g.lda = ld; g.diagA = s->linv;
-            g.B = Pt; g.ldb = np;
-            g.C = M + (int64_t)j * TILE; g.ldc = ld;
-            tg::launch(_ctx, g, (unsigned)(T - 1 - j));
-        }
-    }
+    invert_factor(_ctx, s, linvT);
     const int64_t ntiles = (int64_t)T * (T + 1) / 2;
     Scratch part_buf(_ctx, (size_t)ntiles * KGRAD_MAX_SLOTS * 8), wd_buf(_ctx, (size_t)np * 8),
         xd_buf(_ctx, (size_t)n * ndim * 8), g_buf(_ctx, KGRAD_MAX_SLOTS * 8), dd_buf(_ctx, (size_t)n * 8);
@@ -394,7 +452,8 @@ static int dense_log_probability_grad(b200gp_ctx* ctx, const double* prog, int n
         } else {
             tg::launch(_ctx, g, (unsigned)ntiles);
         }
-        tg::slot_reduce_kernel<<<KGRAD_MAX_SLOTS, 1024, 0, _ctx->stream>>>(part_buf.f64(), ntiles, g_buf.f64());
+        tg::slot_reduce_kernel<<<KGRAD_MAX_SLOTS, 1024, 0, _ctx->stream>>>(part_buf.f64(), ntiles, KGRAD_MAX_SLOTS,
+                                                                          g_buf.f64());
         tg::finish_diag_kernel<<<(unsigned)((n + 255) / 256), 256, 0, _ctx->stream>>>(av, wd_buf.f64(), n, dd_buf.f64());
         _ctx->launches += 2;
         CUDA_CHECK(cudaGetLastError());
@@ -433,6 +492,112 @@ extern "C" int b200gp_dense_log_probability_grad_x(b200gp_ctx* ctx, const double
     }
     return dense_log_probability_grad(ctx, prog, n_instr, X, n, ndim, diag, resid, logp, dprog, dmetric, ddiag, alpha,
                                       dX);
+}
+
+extern "C" int b200gp_dense_fisher(b200gp_ctx* ctx, const double* prog, int n_instr, const double* X, int64_t n,
+                                   int ndim, const double* diag, int with_diag, int* nslot, int* slots, double* fisher) {
+    API_BEGIN(ctx)
+    if (with_diag != 0 && with_diag != 1) throw GpError("fisher: with_diag is 0 or 1");
+    if (nslot == nullptr || slots == nullptr || fisher == nullptr) throw GpError("fisher: nslot, slots and fisher are required");
+    const KProg P = parse_prog(prog, n_instr, ndim);
+    KGrad G;
+    if (!kgrad_prepare(P, G))
+        throw GpError("fisher: the kernel program has more than 16 differentiable parameters, or a leaf without "
+                      "derivatives (closed forms of quasiseparable kernels)");
+    const int S = G.nslot, NP = S + with_diag;
+    const int row0 = n_instr - P.n;    // metric definitions come first
+    *nslot = S;
+    for (int i = 0; i < P.n; ++i) {
+        const int q[2] = {G.slot0[i], G.slot1[i]};
+        for (int c = 0; c < 2; ++c)
+            if (q[c] >= 0) {
+                slots[3 * q[c]] = 0; slots[3 * q[c] + 1] = row0 + i; slots[3 * q[c] + 2] = 2 + c;
+            }
+    }
+    for (int m = 0; m < P.nmetric; ++m)
+        for (int r = 0; r < P.mrows[m]; ++r) {
+            const int q = G.mslot[m] + r;
+            slots[3 * q] = 1; slots[3 * q + 1] = m; slots[3 * q + 2] = r;
+        }
+    _ctx->fuse_resid = nullptr;
+    b200gp_dense* s = dense_factor_from_prog(_ctx, P, X, n, ndim, diag, true);
+    struct Free { b200gp_dense* s; ~Free() { dense_destroy(s); } } free_s{s};
+    if (s->info != 0 || !isfinite(dense_logdet_half(s))) {
+        for (int i = 0; i < NP * NP; ++i) fisher[i] = NAN;
+        return 0;
+    }
+    const int64_t np = s->np, ld = s->np;
+    const int T = (int)(np / TILE);
+    Scratch lt_buf(_ctx, (size_t)T * TILE * TILE * 8);
+    double* const linvT = lt_buf.f64();
+    double* const M = s->mat;
+    invert_factor(_ctx, s, linvT);
+    std::optional<Scratch> wk_buf;
+    try {
+        wk_buf.emplace(_ctx, (size_t)np * np * 8);
+    } catch (const GpError& e) {
+        char buf[384];
+        snprintf(buf, sizeof(buf), "fisher: the %lld x %lld fp64 work buffer (%.2f GB) does not fit next to the factor: %s",
+                 (long long)np, (long long)np, (double)np * (double)np * 8e-9, e.what());
+        throw GpError(buf);
+    }
+    double* const Wk = wk_buf->f64();
+    const int64_t ntiles = (int64_t)T * (T + 1) / 2;
+    Scratch part_buf(_ctx, (size_t)ntiles * KGRAD_MAX_SLOTS * 8), wd_buf(_ctx, (size_t)np * 8),
+        xd_buf(_ctx, (size_t)n * ndim * 8), f_buf(_ctx, (size_t)NP * NP * 8);
+    CUDA_CHECK(cudaMemcpyAsync(xd_buf.p, X, (size_t)n * ndim * 8, cudaMemcpyDefault, _ctx->stream));
+    tg::mirror_lower_kernel<<<dim3((unsigned)(np / 32), (unsigned)(np / 32)), dim3(32, 8), 0, _ctx->stream>>>(M, ld);
+    _ctx->launches++;
+    const dim3 sq_grid((unsigned)(np / 32), (unsigned)(np / 32)), sq_block(32, 8);
+    // Wk <- Wk X^T (RMUL_XT, column blocks descending) or Wk X (RMUL_X, ascending), in place
+    auto rmul = [&](int mode) {
+        for (int jj = 0; jj < T; ++jj) {
+            tg::Args g{};
+            g.mode = mode; g.T = T; g.j = (mode == tg::RMUL_XT) ? T - 1 - jj : jj;
+            g.A = Wk; g.lda = np;
+            g.B = M; g.ldb = ld; g.diagB = (mode == tg::RMUL_XT) ? s->linv : linvT;
+            g.C = Wk; g.ldc = np;
+            tg::launch(_ctx, g, (unsigned)T);
+        }
+    };
+    auto transpose = [&]() {
+        tg::transpose_inplace_kernel<<<sq_grid, sq_block, 0, _ctx->stream>>>(Wk, np);
+        _ctx->launches++;
+    };
+    for (int b = 0; b < NP; ++b) {
+        tg::dk_build_kernel<<<sq_grid, sq_block, 0, _ctx->stream>>>(P, G, xd_buf.f64(), ndim, n, np, b, Wk);
+        _ctx->launches++;
+        rmul(tg::RMUL_XT);
+        transpose();
+        rmul(tg::RMUL_XT);     // E_b = X dK_b X^T
+        rmul(tg::RMUL_X);
+        transpose();
+        rmul(tg::RMUL_X);      // C_b = X^T E_b X
+        tg::Args g{};
+        g.mode = tg::FISHER; g.T = T;
+        g.A = Wk; g.lda = np;
+        g.P = P; g.G = G;
+        g.X = xd_buf.f64(); g.ndim = ndim; g.n = n;
+        g.wdiag = wd_buf.f64(); g.partial = part_buf.f64();
+        tg::launch(_ctx, g, (unsigned)ntiles);
+        double* const row = f_buf.f64() + (int64_t)b * NP;
+        if (S > 0) {
+            tg::slot_reduce_kernel<<<S, 1024, 0, _ctx->stream>>>(part_buf.f64(), ntiles, KGRAD_MAX_SLOTS, row);
+            _ctx->launches++;
+        }
+        if (with_diag) {
+            tg::slot_reduce_kernel<<<1, 1024, 0, _ctx->stream>>>(wd_buf.f64(), n, 1, row + S);   // 1/2 tr(C_b)
+            _ctx->launches++;
+        }
+        CUDA_CHECK(cudaGetLastError());
+    }
+    std::vector<double> fr((size_t)NP * NP);
+    CUDA_CHECK(cudaMemcpyAsync(fr.data(), f_buf.p, fr.size() * 8, cudaMemcpyDeviceToHost, _ctx->stream));
+    CUDA_CHECK(cudaStreamSynchronize(_ctx->stream));
+    // row b holds 1/2 <dK_a, C_b>: both triangles from the mean, so the matrix is symmetric bit for bit
+    for (int a = 0; a < NP; ++a)
+        for (int b = 0; b < NP; ++b) fisher[a * NP + b] = 0.5 * (fr[(size_t)a * NP + b] + fr[(size_t)b * NP + a]);
+    API_END
 }
 
 // ---- diagnostics entry point: one launch of tri_gemm_kernel on host operands, with the Args and grid of

@@ -278,3 +278,21 @@ __host__ __device__ __forceinline__ double kgrad_eval(const KProg& P, const KGra
     }
     return val[P.n - 1];
 }
+
+// element (i, j) of dK / d slot for the Fisher information's derivative build (grad.cu dk_build_kernel), X n x ndim
+// row-major: slot < G.nslot is a program slot, slot == G.nslot the scalar noise diagonal (dK / d diag = I); 0 outside the
+// n x n matrix, so that the padded rows and columns stay 0 through the products by L^-1
+__host__ __device__ __forceinline__ double kgrad_element(const KProg& P, const KGrad& G, int ndim, const double* X,
+                                                         int64_t n, int64_t i, int64_t j, int slot) {
+    if (i >= n || j >= n) return 0.0;
+    if (slot == G.nslot) return (i == j) ? 1.0 : 0.0;
+    const double* xa = X + i * ndim;
+    const double* xb = X + j * ndim;
+    double dk[KGRAD_MAX_SLOTS];
+    kgrad_eval(P, G, ndim, [&](int d) { return xa[d] - xb[d]; }, dk);
+    double v = 0.0;
+#pragma unroll
+    for (int s = 0; s < KGRAD_MAX_SLOTS; ++s)
+        if (s == slot) v = dk[s];
+    return v;
+}

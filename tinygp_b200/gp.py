@@ -6,7 +6,7 @@ the six ``Solver`` methods exactly where the reference calls them (gp.py:120,124
 
 from __future__ import annotations
 
-__all__ = ["GaussianProcess", "ConditionResult", "LogProbabilityGrad", "LogProbabilityGradX"]
+__all__ = ["GaussianProcess", "ConditionResult", "LogProbabilityGrad", "LogProbabilityGradX", "FisherInformation"]
 
 import copy
 from typing import Any, NamedTuple
@@ -102,6 +102,40 @@ class GaussianProcess:
         if wrt_X:
             return logp, LogProbabilityGradX(**fields, X=dX.reshape(np.shape(self.X)))
         return logp, LogProbabilityGrad(**fields)
+
+    def fisher_information(self) -> "FisherInformation":
+        """The expected Fisher information of ``log_probability`` with respect to the kernel's differentiable fields and
+        a scalar ``diag``: F_ab = 1/2 tr(K^-1 dK/da K^-1 dK/db), which does not depend on y.  One device call: the factor,
+        L^-1 in place, then for each parameter b the matrix K^-1 dK/db K^-1 by four triangular products and its
+        contraction with every dK/da.  Its rows and columns are ``params``, the order in which ``log_probability_and_grad``
+        visits the kernel (``FisherInformation.flatten`` reads a gradient in that order), then ``("diag", None)`` when
+        ``diag`` was given as a scalar.  A per-point noise diagonal is not a parameter of F, and neither is the mean.
+
+        Scope and refusals are those of ``log_probability_and_grad``: the dense DirectSolver, a diagonal noise model, at
+        most 16 differentiable scalars; anything else raises NotImplementedError.  A node that occurs twice gets the sum
+        over its occurrences.  A non positive-definite covariance gives an all-NaN matrix.  The solver's own factor is not
+        touched.  Costs about 4 P n^3 flops and one n x n fp64 buffer beyond the gradient's memory (P the device's
+        parameter count).  A Fisher-scoring step is ``np.linalg.solve(F.matrix, F.flatten(grad))``."""
+        hook = getattr(self.solver, "fisher_information", None)
+        if hook is None:
+            raise NotImplementedError(f"fisher_information: not available for {type(self.solver).__name__} (only the "
+                                      "dense DirectSolver)")
+        Fs, rows = hook(self._scalar_diag)
+        entries = list(_param_walk(self.kernel))
+        params = [label for label, _ in entries]
+        column = {key: p for p, (_, key) in enumerate(entries)}
+        if self._scalar_diag:
+            params.append(("diag", None))
+        J = np.zeros((Fs.shape[0], len(params)))      # d slot / d parameter
+        for s, ents in enumerate(rows):
+            for node, field, idx, coef in ents:
+                J[s, column[(id(node), field, idx)]] += coef
+        if self._scalar_diag:
+            J[-1, -1] = 1.0
+        if not np.all(np.isfinite(Fs)):
+            return FisherInformation(np.full((len(params), len(params)), np.nan), params)
+        A = J.T @ Fs @ J
+        return FisherInformation(0.5 * (A + A.T), params)
 
     def condition(self, y, X_test=None, *, diag=None, noise: Noise | None = None, include_mean: bool = True,
                   kernel=None) -> "ConditionResult":
@@ -227,6 +261,51 @@ class LogProbabilityGradX(NamedTuple):
     diag: Any
     mean: np.ndarray
     X: np.ndarray
+
+
+class FisherInformation(NamedTuple):
+    """``GaussianProcess.fisher_information()``: ``matrix`` (P x P, float64, symmetric bit for bit) over ``params``, one
+    label per row: ``(path, None)`` for a scalar field, e.g. ``("kernel1.value", None)``, ``(path, i)`` for entry i of a
+    1-D ``Linear.scale`` / ``Cholesky.factor``, e.g. ``("kernel2.kernel.scale", 1)``, and ``("diag", None)`` last for a
+    scalar ``diag``."""
+    matrix: np.ndarray
+    params: list
+
+    def flatten(self, grad) -> np.ndarray:
+        """a ``LogProbabilityGrad`` (or ``LogProbabilityGradX``) of the same model as a vector in ``params`` order"""
+        entries = list(_param_walk(grad.kernel, values=True))
+        labels = [label for label, _ in entries]
+        has_diag = bool(self.params) and self.params[-1] == ("diag", None)
+        if labels != list(self.params[:len(self.params) - has_diag]):
+            raise ValueError("flatten: the gradient's kernel does not have this Fisher information's parameters")
+        out = [value for _, value in entries]
+        if has_diag:
+            if np.ndim(grad.diag) != 0:
+                raise ValueError("flatten: the Fisher information has a scalar diag, the gradient a per-point one")
+            out.append(float(grad.diag))
+        return np.asarray(out, dtype=np.float64)
+
+
+def _param_walk(node, values=False, path="", memo=None):
+    """(label, key) of every differentiable scalar in the order _grad_tree visits the kernel: depth-first over
+    vars(node), a shared node once, one entry per index of a 1-D field; key = (id(node), field, index or None), or with
+    ``values`` the field's value there"""
+    memo = set() if memo is None else memo
+    if id(node) in memo:
+        return
+    memo.add(id(node))
+    fields = _grad_fields(node)
+    for name, value in vars(node).items():
+        label = path + name
+        if isinstance(value, kernels.Kernel):
+            yield from _param_walk(value, values, label + ".", memo)
+        elif name in fields:
+            if np.ndim(value) == 0:
+                yield (label, None), (float(value) if values else (id(node), name, None))
+            else:
+                flat = np.asarray(value, dtype=np.float64).reshape(-1)
+                for i in range(flat.shape[0]):
+                    yield (label, i), (float(flat[i]) if values else (id(node), name, i))
 
 
 def _grad_fields(node) -> tuple[str, ...]:

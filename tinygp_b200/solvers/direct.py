@@ -184,6 +184,52 @@ class DirectSolver(Solver):
             return logp.value, grads, ddiag, alpha, dX
         return logp.value, grads, ddiag, alpha
 
+    def fisher_information(self, with_diag: bool):
+        """The expected Fisher information over the device's slots (b200gp_dense_fisher), with a factor of its own: the
+        solver's factor, built or pending, is left as it is.  ``with_diag``: one more slot, last, for a scalar noise
+        diagonal (dK / d diag = I).  Returns (F, rows): F of shape (S + with_diag, S + with_diag), and for each program
+        slot s the list rows[s] of (node, field, index, d slot / d field) that map it to the kernel's fields (index None
+        for a scalar field) -- the slot-to-field map of log_probability_grad."""
+        if self._x is None:
+            what = ("noise.Dense / noise.Banded" if not isinstance(self.noise, Diagonal)
+                    else "a precomputed covariance (covariance=) or a kernel without a device program")
+            raise NotImplementedError(f"fisher_information: not available for {what}; only kernel programs with a "
+                                      "diagonal noise model are differentiated on the device")
+        try:
+            prog, x, leaves, owners = self.kernel.lower_for_grad(self.X)
+        except NotImplementedError as e:
+            raise NotImplementedError(f"fisher_information: {e}") from e
+        nslot = sum(2 if p1 is not None else 1 for _, _, p1 in leaves) + sum(len(o) for o in owners)
+        if nslot > MAX_GRAD_SLOTS:
+            raise NotImplementedError(f"fisher_information: the kernel has {nslot} differentiable scalars (leaf scales, "
+                                      f"constants, gamma / alpha, transform rows); at most {MAX_GRAD_SLOTS} are supported")
+        ns = c_int()
+        slots = np.zeros(3 * MAX_GRAD_SLOTS, dtype=np.int32)
+        F = np.empty((MAX_GRAD_SLOTS + 1) ** 2)
+        self._ctx.check(self._ctx.lib.b200gp_dense_fisher(self._ctx.handle, _cabi.ptr(prog), prog.shape[0], _cabi.ptr(x),
+                                                          x.shape[0], x.shape[1], _cabi.ptr(self._diag), int(bool(with_diag)),
+                                                          byref(ns), _cabi.ptr(slots), _cabi.ptr(F)))
+        k = ns.value + int(bool(with_diag))
+        F = F[:k * k].reshape(k, k).copy()
+        n_instr = 2 * len(leaves) - 1      # leaves and the binary ADD / MUL over them, after the metric rows
+        ops = prog[-n_instr:, 0]
+        leaf_rows = prog.shape[0] - n_instr + np.flatnonzero((ops != OP_ADD) & (ops != OP_MUL))
+        leaf_at = dict(zip(leaf_rows.tolist(), leaves))
+        rows = []
+        for kind, a, b in slots[:3 * ns.value].reshape(-1, 3).tolist():
+            if kind == 0:
+                node, f0, f1 = leaf_at[a]
+                rows.append([(node, f0 if b == 2 else f1, None, 1.0)])
+                continue
+            ents = []
+            for node, field, idx, how in owners[a][b]:   # row scale lambda -> d lambda / d s_r = 1 / s_r, -1 / f_r
+                v = np.asarray(getattr(node, field), dtype=np.float64)
+                s = float(v) if v.ndim == 0 else float(v[idx])
+                ents.append((node, field, None if v.ndim == 0 else idx,
+                             0.0 if s == 0.0 else (1.0 / s if how == "linear" else -1.0 / s)))
+            rows.append(ents)
+        return F, rows
+
     def __del__(self):
         h = getattr(self, "_h", None)
         if h:
