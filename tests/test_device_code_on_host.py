@@ -5,14 +5,13 @@ here is the launch geometry and memory system, which the `-m gpu` tests cover.""
 
 import ctypes
 import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
 from oracle import tinygp_np as o
 from tinygp_b200.kernels import quasisep as Q
+from util import host_library
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "csrc", "qs_hostcheck.cu")
@@ -54,14 +53,7 @@ KERNELS = {
 
 @pytest.fixture(scope="module")
 def lib():
-    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    if not os.path.exists(nvcc):
-        pytest.skip("nvcc not available")
-    if not os.path.exists(OUT) or any(os.path.getmtime(d) > os.path.getmtime(OUT) for d in DEPS):
-        os.makedirs(os.path.dirname(OUT), exist_ok=True)
-        subprocess.run([nvcc, "-O2", "-std=c++17", "-Wno-deprecated-gpu-targets", "-Xcompiler", "-fPIC", "-shared",
-                        "-o", OUT, SRC], check=True)
-    return ctypes.CDLL(OUT)
+    return host_library(SRC, OUT, DEPS)
 
 
 def _p(a):
@@ -130,14 +122,7 @@ KDEPS = [KSRC, os.path.join(HERE, "..", "tinygp_b200", "csrc", "kprog.cuh"),
 
 @pytest.fixture(scope="module")
 def klib():
-    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    if not os.path.exists(nvcc):
-        pytest.skip("nvcc not available")
-    if not os.path.exists(KOUT) or any(os.path.getmtime(d) > os.path.getmtime(KOUT) for d in KDEPS):
-        os.makedirs(os.path.dirname(KOUT), exist_ok=True)
-        subprocess.run([nvcc, "-O2", "-std=c++17", "-Wno-deprecated-gpu-targets", "-diag-suppress", "20013",
-                        "-Xcompiler", "-fPIC", "-shared", "-o", KOUT, KSRC], check=True)
-    return ctypes.CDLL(KOUT)
+    return host_library(KSRC, KOUT, KDEPS, ["-diag-suppress", "20013"])
 
 
 def _kmat(klib, k, X1, X2):

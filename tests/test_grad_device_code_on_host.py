@@ -5,8 +5,6 @@ forms (oracle/grad_np.py)."""
 
 import ctypes
 import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -14,6 +12,7 @@ import pytest
 from oracle import grad_np
 from oracle import tinygp_np as o
 from tinygp_b200 import kernels, transforms
+from util import host_library
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "csrc", "kgrad_hostcheck.cu")
@@ -25,14 +24,7 @@ P = ctypes.c_void_p
 
 @pytest.fixture(scope="module")
 def lib():
-    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    if not os.path.exists(nvcc):
-        pytest.skip("nvcc not available")
-    if not os.path.exists(OUT) or any(os.path.getmtime(d) > os.path.getmtime(OUT) for d in DEPS):
-        os.makedirs(os.path.dirname(OUT), exist_ok=True)
-        subprocess.run([nvcc, "-O2", "-std=c++17", "-Wno-deprecated-gpu-targets", "-diag-suppress", "20013",
-                        "-Xcompiler", "-fPIC", "-shared", "-o", OUT, SRC], check=True)
-    return ctypes.CDLL(OUT)
+    return host_library(SRC, OUT, DEPS, ["-diag-suppress", "20013"])
 
 
 def _ptr(a):

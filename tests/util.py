@@ -1,6 +1,13 @@
-"""Shared helpers for the parity tests: map a product kernel expression onto the oracle's classes."""
+"""Shared helpers for the parity tests: map a product kernel expression onto the oracle's classes; build the device
+source checks of tests/csrc for the CPU."""
+
+import ctypes
+import os
+import shutil
+import subprocess
 
 import numpy as np
+import pytest
 
 from oracle import tinygp_np as o
 from tinygp_b200 import kernels as K
@@ -49,3 +56,16 @@ def assert_close(a, b, rtol=FP64_RTOL, atol=FP64_RTOL):
 
 def rel(a, b):
     return abs(a - b) / abs(b)
+
+
+def host_library(src, out, deps, flags=()):
+    """``src`` (a tests/csrc/*_hostcheck.cu) compiled for the CPU by nvcc into the shared library ``out``, loaded with
+    ctypes; rebuilt when ``out`` is older than one of ``deps``.  Skips the calling test when nvcc is not installed."""
+    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
+    if not os.path.exists(nvcc):
+        pytest.skip("nvcc not available")
+    if not os.path.exists(out) or any(os.path.getmtime(d) > os.path.getmtime(out) for d in deps):
+        os.makedirs(os.path.dirname(out), exist_ok=True)
+        subprocess.run([nvcc, "-O2", "-std=c++17", "-Wno-deprecated-gpu-targets", *flags, "-Xcompiler", "-fPIC", "-shared",
+                        "-o", out, src], check=True)
+    return ctypes.CDLL(out)

@@ -341,32 +341,115 @@ static void launch(b200gp_ctx* ctx, const Args& g, unsigned nblocks) {
     CUDA_CHECK(cudaGetLastError());
     ctx->launches++;
 }
+
+// step 2's launch for block column j < T - 1: C_ij = sum_{k=j+1..i} A_ik B_k^T for i > j, A's diagonal blocks from
+// diagA, B 128 rows; every matrix np = 128 T columns wide
+static void trmm(b200gp_ctx* ctx, int T, int j, const double* A, const double* diagA, const double* B, double* C) {
+    Args g{};
+    g.mode = TRMM; g.j = j; g.T = T;
+    g.A = A; g.lda = (int64_t)T * TILE; g.diagA = diagA;
+    g.B = B; g.ldb = (int64_t)T * TILE;
+    g.C = C + (int64_t)j * TILE; g.ldc = (int64_t)T * TILE;
+    launch(ctx, g, (unsigned)(T - 1 - j));
+}
+
+// step 3's launch: the lower tiles of W = U U^T, U = A (np x np, np = 128 T) with its diagonal blocks from diagA, and
+// the CONTRACT epilogue over them.  dxpart != nullptr: the coordinate gradient too (tri_gemm_kernel<true>), reduced per
+// point into dX.
+static void contract(b200gp_ctx* ctx, int T, const double* A, const double* diagA, const KProg& P, const KGrad& G,
+                     const double* X, int ndim, int64_t n, const double* alphav, double* wdiag, double* partial,
+                     double* dxpart, double* dX) {
+    Args g{};
+    g.mode = CONTRACT; g.T = T;
+    g.A = A; g.lda = (int64_t)T * TILE; g.diagA = diagA;
+    g.B = A; g.ldb = (int64_t)T * TILE; g.diagB = diagA;
+    g.P = P; g.G = G;
+    g.X = X; g.ndim = ndim; g.n = n;
+    g.alphav = alphav; g.wdiag = wdiag; g.partial = partial;
+    const unsigned ntiles = (unsigned)((int64_t)T * (T + 1) / 2);
+    if (dxpart == nullptr) {
+        launch(ctx, g, ntiles);
+        return;
+    }
+    g.dxpart = dxpart;
+    launch<true>(ctx, g, ntiles);
+    dx_reduce_kernel<<<dim3((unsigned)T, (unsigned)ndim), BM, 0, ctx->stream>>>(dxpart, T, ndim, n, dX);
+    CUDA_CHECK(cudaGetLastError());
+    ctx->launches++;
+}
 }  // namespace tg
 
-// step 2: X = L^-1 in place in the lower block triangle of s->mat (its diagonal blocks stay in s->linv); linvT <- the
-// diagonal blocks transposed (T x 128 x 128)
-static void invert_factor(b200gp_ctx* _ctx, b200gp_dense* s, double* linvT) {
+// the kernel program and its slot layout for kgrad_eval; a program without device derivatives is refused, the message
+// prefixed by `who`
+static void parse_for_grad(const char* who, const double* prog, int n_instr, int ndim, KProg& P, KGrad& G) {
+    P = parse_prog(prog, n_instr, ndim);
+    if (!kgrad_prepare(P, G))
+        throw GpError(std::string(who) + ": the kernel program has more than 16 differentiable parameters, or a leaf "
+                      "without derivatives (closed forms of quasiseparable kernels)");
+}
+
+// step 1 of the gradient and the Fisher information: the program parsed for kgrad_eval, and the factor of
+// b200gp_dense_log_probability without its fused forward substitution (alpha needs both solves), freed with this object
+struct GradFactor {
+    KProg P;
+    KGrad G;
+    b200gp_dense* s;
+    GradFactor(b200gp_ctx* ctx, const char* who, const double* prog, int n_instr, const double* X, int64_t n, int ndim,
+               const double* diag) {
+        parse_for_grad(who, prog, n_instr, ndim, P, G);
+        ctx->fuse_resid = nullptr;
+        s = dense_factor_from_prog(ctx, P, X, n, ndim, diag, true);
+    }
+    ~GradFactor() { dense_destroy(s); }
+    GradFactor(const GradFactor&) = delete;
+    GradFactor& operator=(const GradFactor&) = delete;
+};
+
+// what slot q of kgrad_prepare's layout differentiates, as o[0..2]: {0, program row, column 2 (p0) or 3 (p1)} for an
+// instruction's parameter, {1, metric m, row r} for a row scale of a metric (n_rows: program rows, metric definitions
+// first)
+static void slot_origin(const KProg& P, const KGrad& G, int n_rows, int q, int* o) {
+    for (int i = 0; i < P.n; ++i)
+        if (G.slot0[i] == q || G.slot1[i] == q) {
+            o[0] = 0; o[1] = n_rows - P.n + i; o[2] = (G.slot0[i] == q) ? 2 : 3;
+            return;
+        }
+    for (int m = 0; m < P.nmetric; ++m)
+        if (q >= G.mslot[m] && q < G.mslot[m] + P.mrows[m]) {
+            o[0] = 1; o[1] = m; o[2] = q - G.mslot[m];
+            return;
+        }
+}
+
+// steps 2 and 3's operands: X = L^-1 in place in the lower block triangle of s->mat (its diagonal blocks stay in
+// s->linv), linvT <- the diagonal blocks transposed (T x 128 x 128), U = X^T mirrored into the upper triangle, and xd <-
+// the n x ndim coordinates X (host or device).  The mirror and the upload count toward the profile field `prof`
+// (nullptr: toward none).
+static void invert_factor(b200gp_ctx* _ctx, b200gp_dense* s, double* linvT, const double* X, int64_t n, int ndim,
+                          double* xd, double* prof) {
     const int64_t np = s->np, ld = s->np;
     const int T = (int)(np / TILE);
     double* const M = s->mat;
-    Scratch pt_buf(_ctx, (size_t)TILE * np * 8);
-    double* const Pt = pt_buf.f64();
-    tg::block_transpose_kernel<<<dim3(TILE / 32, TILE / 32, T), dim3(32, 8), 0, _ctx->stream>>>(s->linv, linvT);
-    _ctx->launches++;
-    // X = L^-1 in place: for j = T-2 .. 0,  X_ij = sum_{k=j+1..i} X_ik (-L_kj X_jj)  for i > j;  X_jj = linv_j
-    ProfTimer t(_ctx, &_ctx->prof.trtri_ms);
-    for (int j = T - 2; j >= 0; --j) {
-        // Pt (128 x np, column blocks k > j) = -(L_kj X_jj)^T = -X_jj^T L_kj^T
-        gemm_nt(_ctx, Pt + (int64_t)(j + 1) * TILE, np, linvT + (int64_t)j * TILE * TILE, TILE,
-                M + (int64_t)(j + 1) * TILE * ld + (int64_t)j * TILE, ld, 1, T - 1 - j, TILE, -1.0, 0, 0);
-        // block column j below the diagonal <- X_{i, j+1..i} Pt^T (diagonal blocks of X from linv)
-        tg::Args g{};
-        g.mode = tg::TRMM; g.j = j; g.T = T;
-        g.A = M; g.lda = ld; g.diagA = s->linv;
-        g.B = Pt; g.ldb = np;
-        g.C = M + (int64_t)j * TILE; g.ldc = ld;
-        tg::launch(_ctx, g, (unsigned)(T - 1 - j));
+    {
+        Scratch pt_buf(_ctx, (size_t)TILE * np * 8);
+        double* const Pt = pt_buf.f64();
+        tg::block_transpose_kernel<<<dim3(TILE / 32, TILE / 32, T), dim3(32, 8), 0, _ctx->stream>>>(s->linv, linvT);
+        _ctx->launches++;
+        // X = L^-1 in place: for j = T-2 .. 0,  X_ij = sum_{k=j+1..i} X_ik (-L_kj X_jj)  for i > j;  X_jj = linv_j
+        ProfTimer t(_ctx, &_ctx->prof.trtri_ms);
+        for (int j = T - 2; j >= 0; --j) {
+            // Pt (128 x np, column blocks k > j) = -(L_kj X_jj)^T = -X_jj^T L_kj^T
+            gemm_nt(_ctx, Pt + (int64_t)(j + 1) * TILE, np, linvT + (int64_t)j * TILE * TILE, TILE,
+                    M + (int64_t)(j + 1) * TILE * ld + (int64_t)j * TILE, ld, 1, T - 1 - j, TILE, -1.0, 0, 0);
+            // block column j below the diagonal <- X_{i, j+1..i} Pt^T (diagonal blocks of X from linv)
+            tg::trmm(_ctx, T, j, M, s->linv, Pt, M);
+        }
     }
+    std::optional<ProfTimer> t;
+    if (prof != nullptr) t.emplace(_ctx, prof);
+    tg::mirror_lower_kernel<<<dim3((unsigned)(np / 32), (unsigned)(np / 32)), dim3(32, 8), 0, _ctx->stream>>>(M, ld);
+    _ctx->launches++;
+    CUDA_CHECK(cudaMemcpyAsync(xd, X, (size_t)n * ndim * 8, cudaMemcpyDefault, _ctx->stream));
 }
 
 // both entry points; dX == nullptr: the plain gradient (tri_gemm_kernel<false>)
@@ -374,18 +457,13 @@ static int dense_log_probability_grad(b200gp_ctx* ctx, const double* prog, int n
                                       int ndim, const double* diag, const double* resid, double* logp, double* dprog,
                                       double* dmetric, double* ddiag, double* alpha, double* dX) {
     API_BEGIN(ctx)
-    const KProg P = parse_prog(prog, n_instr, ndim);
     if (dX != nullptr && (ndim < 1 || ndim > KGRAD_MAX_DIM))
         throw GpError("log_probability_grad_x: coordinate gradients support 1 to 8 input dimensions");
-    KGrad G;
-    if (!kgrad_prepare(P, G))
-        throw GpError("log_probability_grad: the kernel program has more than 16 differentiable parameters, or a leaf "
-                      "without derivatives (closed forms of quasiseparable kernels)");
-    // the factor of b200gp_dense_log_probability, without its fused forward substitution (alpha needs both solves)
-    _ctx->fuse_resid = nullptr;
-    b200gp_dense* s = dense_factor_from_prog(_ctx, P, X, n, ndim, diag, true);
-    struct Free { b200gp_dense* s; ~Free() { dense_destroy(s); } } free_s{s};
-    const int64_t np = s->np, ld = s->np;
+    const GradFactor f(_ctx, "log_probability_grad", prog, n_instr, X, n, ndim, diag);
+    const KProg& P = f.P;
+    const KGrad& G = f.G;
+    b200gp_dense* const s = f.s;
+    const int64_t np = s->np;
     const int T = (int)(np / TILE);
     Scratch y_buf(_ctx, (size_t)np * 8), x_buf(_ctx, (size_t)np * 8), a_buf(_ctx, (size_t)np * 8);
     double* const yv = y_buf.f64();
@@ -397,13 +475,12 @@ static int dense_log_probability_grad(b200gp_ctx* ctx, const double* prog, int n
     const double ss = dense_sumsq_dev(_ctx, xv, n);
     const double ldh = dense_logdet_half(s);
     double lp = -0.5 * ss - (ldh + 0.5 * (double)n * log(2.0 * M_PI));   // gp.py:313-316, direct.py:61-64
-    const int nrows = n_instr;
-    for (int i = 0; i < nrows * B200GP_PROG_STRIDE; ++i) dprog[i] = 0.0;
+    for (int i = 0; i < n_instr * B200GP_PROG_STRIDE; ++i) dprog[i] = 0.0;
     for (int i = 0; i < B200GP_PROG_MAX_METRICS * B200GP_METRIC_MAX_DIM; ++i) dmetric[i] = 0.0;
     if (s->info != 0 || !isfinite(lp)) {
         *logp = -INFINITY;
         const double nan = NAN;
-        const int row0 = nrows - P.n;
+        const int row0 = n_instr - P.n;    // metric definitions come first
         for (int i = 0; i < P.n; ++i)
             for (int q = 2; q < 4; ++q) dprog[(row0 + i) * B200GP_PROG_STRIDE + q] = nan;
         for (int m = 0; m < P.nmetric; ++m)
@@ -417,14 +494,11 @@ static int dense_log_probability_grad(b200gp_ctx* ctx, const double* prog, int n
     CUDA_CHECK(cudaMemcpyAsync(yv, xv, (size_t)np * 8, cudaMemcpyDeviceToDevice, _ctx->stream));
     dense_solve_vec_dev(s, yv, av, true);                                  // alpha = L^-T L^-1 r (pad rows: 0)
 
-    const size_t blk_bytes = (size_t)T * TILE * TILE * 8;
-    Scratch lt_buf(_ctx, blk_bytes);
-    double* const linvT = lt_buf.f64();
-    double* const M = s->mat;
-    invert_factor(_ctx, s, linvT);
+    Scratch lt_buf(_ctx, (size_t)T * TILE * TILE * 8), xd_buf(_ctx, (size_t)n * ndim * 8);
+    invert_factor(_ctx, s, lt_buf.f64(), X, n, ndim, xd_buf.f64(), &_ctx->prof.contract_ms);
     const int64_t ntiles = (int64_t)T * (T + 1) / 2;
     Scratch part_buf(_ctx, (size_t)ntiles * KGRAD_MAX_SLOTS * 8), wd_buf(_ctx, (size_t)np * 8),
-        xd_buf(_ctx, (size_t)n * ndim * 8), g_buf(_ctx, KGRAD_MAX_SLOTS * 8), dd_buf(_ctx, (size_t)n * 8);
+        g_buf(_ctx, KGRAD_MAX_SLOTS * 8), dd_buf(_ctx, (size_t)n * 8);
     const bool want_dx = dX != nullptr;
     std::optional<Scratch> dxp_buf, dx_buf;
     if (want_dx) {
@@ -433,25 +507,9 @@ static int dense_log_probability_grad(b200gp_ctx* ctx, const double* prog, int n
     }
     {
         ProfTimer t(_ctx, &_ctx->prof.contract_ms);
-        tg::mirror_lower_kernel<<<dim3((unsigned)(np / 32), (unsigned)(np / 32)), dim3(32, 8), 0, _ctx->stream>>>(M, ld);
-        _ctx->launches++;
-        CUDA_CHECK(cudaMemcpyAsync(xd_buf.p, X, (size_t)n * ndim * 8, cudaMemcpyDefault, _ctx->stream));
-        tg::Args g{};
-        g.mode = tg::CONTRACT; g.T = T;
-        g.A = M; g.lda = ld; g.diagA = linvT;        // rows of U = X^T; U's diagonal blocks are linv^T
-        g.B = M; g.ldb = ld; g.diagB = linvT;
-        g.P = P; g.G = G;
-        g.X = xd_buf.f64(); g.ndim = ndim; g.n = n;
-        g.alphav = av; g.wdiag = wd_buf.f64(); g.partial = part_buf.f64();
-        if (want_dx) {
-            g.dxpart = dxp_buf->f64();
-            tg::launch<true>(_ctx, g, (unsigned)ntiles);
-            tg::dx_reduce_kernel<<<dim3((unsigned)T, (unsigned)ndim), tg::BM, 0, _ctx->stream>>>(dxp_buf->f64(), T, ndim, n,
-                                                                                           dx_buf->f64());
-            _ctx->launches++;
-        } else {
-            tg::launch(_ctx, g, (unsigned)ntiles);
-        }
+        // rows of U = X^T; U's diagonal blocks are linv^T
+        tg::contract(_ctx, T, s->mat, lt_buf.f64(), P, G, xd_buf.f64(), ndim, n, av, wd_buf.f64(), part_buf.f64(),
+                     want_dx ? dxp_buf->f64() : nullptr, want_dx ? dx_buf->f64() : nullptr);
         tg::slot_reduce_kernel<<<KGRAD_MAX_SLOTS, 1024, 0, _ctx->stream>>>(part_buf.f64(), ntiles, KGRAD_MAX_SLOTS,
                                                                           g_buf.f64());
         tg::finish_diag_kernel<<<(unsigned)((n + 255) / 256), 256, 0, _ctx->stream>>>(av, wd_buf.f64(), n, dd_buf.f64());
@@ -464,13 +522,11 @@ static int dense_log_probability_grad(b200gp_ctx* ctx, const double* prog, int n
     CUDA_CHECK(cudaMemcpyAsync(alpha, av, (size_t)n * 8, cudaMemcpyDeviceToHost, _ctx->stream));
     if (want_dx) CUDA_CHECK(cudaMemcpyAsync(dX, dx_buf->p, (size_t)n * ndim * 8, cudaMemcpyDeviceToHost, _ctx->stream));
     CUDA_CHECK(cudaStreamSynchronize(_ctx->stream));
-    const int row0 = nrows - P.n;      // metric definitions come first
-    for (int i = 0; i < P.n; ++i) {
-        if (G.slot0[i] >= 0) dprog[(row0 + i) * B200GP_PROG_STRIDE + 2] = gh[G.slot0[i]];
-        if (G.slot1[i] >= 0) dprog[(row0 + i) * B200GP_PROG_STRIDE + 3] = gh[G.slot1[i]];
+    for (int q = 0; q < G.nslot; ++q) {
+        int o[3];
+        slot_origin(P, G, n_instr, q, o);
+        (o[0] == 0 ? dprog[o[1] * B200GP_PROG_STRIDE + o[2]] : dmetric[o[1] * B200GP_METRIC_MAX_DIM + o[2]]) = gh[q];
     }
-    for (int m = 0; m < P.nmetric; ++m)
-        for (int r = 0; r < P.mrows[m]; ++r) dmetric[m * B200GP_METRIC_MAX_DIM + r] = gh[G.mslot[m] + r];
     API_END
 }
 
@@ -499,39 +555,23 @@ extern "C" int b200gp_dense_fisher(b200gp_ctx* ctx, const double* prog, int n_in
     API_BEGIN(ctx)
     if (with_diag != 0 && with_diag != 1) throw GpError("fisher: with_diag is 0 or 1");
     if (nslot == nullptr || slots == nullptr || fisher == nullptr) throw GpError("fisher: nslot, slots and fisher are required");
-    const KProg P = parse_prog(prog, n_instr, ndim);
-    KGrad G;
-    if (!kgrad_prepare(P, G))
-        throw GpError("fisher: the kernel program has more than 16 differentiable parameters, or a leaf without "
-                      "derivatives (closed forms of quasiseparable kernels)");
+    const GradFactor f(_ctx, "fisher", prog, n_instr, X, n, ndim, diag);
+    const KProg& P = f.P;
+    const KGrad& G = f.G;
+    b200gp_dense* const s = f.s;
     const int S = G.nslot, NP = S + with_diag;
-    const int row0 = n_instr - P.n;    // metric definitions come first
     *nslot = S;
-    for (int i = 0; i < P.n; ++i) {
-        const int q[2] = {G.slot0[i], G.slot1[i]};
-        for (int c = 0; c < 2; ++c)
-            if (q[c] >= 0) {
-                slots[3 * q[c]] = 0; slots[3 * q[c] + 1] = row0 + i; slots[3 * q[c] + 2] = 2 + c;
-            }
-    }
-    for (int m = 0; m < P.nmetric; ++m)
-        for (int r = 0; r < P.mrows[m]; ++r) {
-            const int q = G.mslot[m] + r;
-            slots[3 * q] = 1; slots[3 * q + 1] = m; slots[3 * q + 2] = r;
-        }
-    _ctx->fuse_resid = nullptr;
-    b200gp_dense* s = dense_factor_from_prog(_ctx, P, X, n, ndim, diag, true);
-    struct Free { b200gp_dense* s; ~Free() { dense_destroy(s); } } free_s{s};
+    for (int q = 0; q < S; ++q) slot_origin(P, G, n_instr, q, slots + 3 * q);
     if (s->info != 0 || !isfinite(dense_logdet_half(s))) {
         for (int i = 0; i < NP * NP; ++i) fisher[i] = NAN;
         return 0;
     }
     const int64_t np = s->np, ld = s->np;
     const int T = (int)(np / TILE);
-    Scratch lt_buf(_ctx, (size_t)T * TILE * TILE * 8);
+    Scratch lt_buf(_ctx, (size_t)T * TILE * TILE * 8), xd_buf(_ctx, (size_t)n * ndim * 8);
     double* const linvT = lt_buf.f64();
     double* const M = s->mat;
-    invert_factor(_ctx, s, linvT);
+    invert_factor(_ctx, s, linvT, X, n, ndim, xd_buf.f64(), nullptr);
     std::optional<Scratch> wk_buf;
     try {
         wk_buf.emplace(_ctx, (size_t)np * np * 8);
@@ -544,10 +584,7 @@ extern "C" int b200gp_dense_fisher(b200gp_ctx* ctx, const double* prog, int n_in
     double* const Wk = wk_buf->f64();
     const int64_t ntiles = (int64_t)T * (T + 1) / 2;
     Scratch part_buf(_ctx, (size_t)ntiles * KGRAD_MAX_SLOTS * 8), wd_buf(_ctx, (size_t)np * 8),
-        xd_buf(_ctx, (size_t)n * ndim * 8), f_buf(_ctx, (size_t)NP * NP * 8);
-    CUDA_CHECK(cudaMemcpyAsync(xd_buf.p, X, (size_t)n * ndim * 8, cudaMemcpyDefault, _ctx->stream));
-    tg::mirror_lower_kernel<<<dim3((unsigned)(np / 32), (unsigned)(np / 32)), dim3(32, 8), 0, _ctx->stream>>>(M, ld);
-    _ctx->launches++;
+        f_buf(_ctx, (size_t)NP * NP * 8);
     const dim3 sq_grid((unsigned)(np / 32), (unsigned)(np / 32)), sq_block(32, 8);
     // Wk <- Wk X^T (RMUL_XT, column blocks descending) or Wk X (RMUL_X, ascending), in place
     auto rmul = [&](int mode) {
@@ -600,9 +637,9 @@ extern "C" int b200gp_dense_fisher(b200gp_ctx* ctx, const double* prog, int n_in
     API_END
 }
 
-// ---- diagnostics entry point: one launch of tri_gemm_kernel on host operands, with the Args and grid of
-// dense_log_probability_grad (include/b200gp.h).  Every size is checked before anything is allocated, so that the
-// kernels read and write only the buffers allocated here.
+// ---- diagnostics entry point: one launch of tri_gemm_kernel on host operands through the launchers of
+// dense_log_probability_grad (tg::trmm, tg::contract; include/b200gp.h).  Every size is checked before anything is
+// allocated, so that the kernels read and write only the buffers allocated here.
 extern "C" int b200gp_grad_tiles_test(b200gp_ctx* ctx, int mode, int T, int j, const double* A, const double* diagA,
                                       const double* B, double* C, const double* prog, int n_instr, const double* X,
                                       int64_t n, int ndim, const double* alpha, double* wdiag, double* partial,
@@ -621,12 +658,7 @@ extern "C" int b200gp_grad_tiles_test(b200gp_ctx* ctx, int mode, int T, int j, c
         CUDA_CHECK(cudaMemcpyAsync(d_buf.p, diagA, blk_bytes, cudaMemcpyHostToDevice, _ctx->stream));
         CUDA_CHECK(cudaMemcpyAsync(b_buf.p, B, b_bytes, cudaMemcpyHostToDevice, _ctx->stream));
         CUDA_CHECK(cudaMemcpyAsync(c_buf.p, C, sq_bytes, cudaMemcpyHostToDevice, _ctx->stream));
-        tg::Args g{};
-        g.mode = tg::TRMM; g.j = j; g.T = T;
-        g.A = a_buf.f64(); g.lda = np; g.diagA = d_buf.f64();
-        g.B = b_buf.f64(); g.ldb = np;
-        g.C = c_buf.f64() + (int64_t)j * TILE; g.ldc = np;
-        tg::launch(_ctx, g, (unsigned)(T - 1 - j));
+        tg::trmm(_ctx, T, j, a_buf.f64(), d_buf.f64(), b_buf.f64(), c_buf.f64());
         CUDA_CHECK(cudaMemcpyAsync(C, c_buf.p, sq_bytes, cudaMemcpyDeviceToHost, _ctx->stream));
         CUDA_CHECK(cudaStreamSynchronize(_ctx->stream));
         return 0;
@@ -637,11 +669,9 @@ extern "C" int b200gp_grad_tiles_test(b200gp_ctx* ctx, int mode, int T, int j, c
     if (prog == nullptr || X == nullptr || alpha == nullptr || wdiag == nullptr || partial == nullptr)
         throw GpError("grad tiles test: CONTRACT needs prog, X, alpha, wdiag and partial");
     if ((dxpart == nullptr) != (dX == nullptr)) throw GpError("grad tiles test: dxpart and dX go together");
-    const KProg P = parse_prog(prog, n_instr, ndim);
+    KProg P;
     KGrad G;
-    if (!kgrad_prepare(P, G))
-        throw GpError("grad tiles test: the kernel program has more than 16 differentiable parameters, or a leaf "
-                      "without derivatives");
+    parse_for_grad("grad tiles test", prog, n_instr, ndim, P, G);
     const bool want_dx = dX != nullptr;
     const int64_t ntiles = (int64_t)T * (T + 1) / 2;
     const size_t part_bytes = (size_t)ntiles * KGRAD_MAX_SLOTS * 8, dxp_bytes = (size_t)ntiles * 2 * ndim * TILE * 8,
@@ -658,24 +688,11 @@ extern "C" int b200gp_grad_tiles_test(b200gp_ctx* ctx, int mode, int T, int j, c
     CUDA_CHECK(cudaMemcpyAsync(x_buf.p, X, x_bytes, cudaMemcpyHostToDevice, _ctx->stream));
     CUDA_CHECK(cudaMemsetAsync(al_buf.p, 0, (size_t)np * 8, _ctx->stream));
     CUDA_CHECK(cudaMemcpyAsync(al_buf.p, alpha, (size_t)n * 8, cudaMemcpyHostToDevice, _ctx->stream));
-    tg::Args g{};
-    g.mode = tg::CONTRACT; g.T = T;
-    g.A = a_buf.f64(); g.lda = np; g.diagA = d_buf.f64();
-    g.B = a_buf.f64(); g.ldb = np; g.diagB = d_buf.f64();
-    g.P = P; g.G = G;
-    g.X = x_buf.f64(); g.ndim = ndim; g.n = n;
-    g.alphav = al_buf.f64(); g.wdiag = wd_buf.f64(); g.partial = part_buf.f64();
+    tg::contract(_ctx, T, a_buf.f64(), d_buf.f64(), P, G, x_buf.f64(), ndim, n, al_buf.f64(), wd_buf.f64(),
+                 part_buf.f64(), want_dx ? dxp_buf->f64() : nullptr, want_dx ? dx_buf->f64() : nullptr);
     if (want_dx) {
-        g.dxpart = dxp_buf->f64();
-        tg::launch<true>(_ctx, g, (unsigned)ntiles);
-        tg::dx_reduce_kernel<<<dim3((unsigned)T, (unsigned)ndim), tg::BM, 0, _ctx->stream>>>(dxp_buf->f64(), T, ndim, n,
-                                                                                       dx_buf->f64());
-        CUDA_CHECK(cudaGetLastError());
-        _ctx->launches++;
         CUDA_CHECK(cudaMemcpyAsync(dxpart, dxp_buf->p, dxp_bytes, cudaMemcpyDeviceToHost, _ctx->stream));
         CUDA_CHECK(cudaMemcpyAsync(dX, dx_buf->p, x_bytes, cudaMemcpyDeviceToHost, _ctx->stream));
-    } else {
-        tg::launch(_ctx, g, (unsigned)ntiles);
     }
     CUDA_CHECK(cudaMemcpyAsync(wdiag, wd_buf.p, (size_t)n * 8, cudaMemcpyDeviceToHost, _ctx->stream));
     CUDA_CHECK(cudaMemcpyAsync(partial, part_buf.p, part_bytes, cudaMemcpyDeviceToHost, _ctx->stream));

@@ -20,6 +20,17 @@ MAX_GRAD_SLOTS = 16     # differentiable scalars per kernel program (KGRAD_MAX_S
 MAX_GRAD_DIM = 8        # input dimensions of gradients with respect to X (KGRAD_MAX_DIM, tinygp_b200/csrc/kgrad.cuh)
 
 
+def _through_row_scale(value, s, kind):
+    """``value`` per unit of a slot, carried to the field that moves it: unchanged where the slot is the field (kind
+    None); through a row scale lambda, value * d lambda / d s_r = value / s_r (Linear), -value / f_r (Cholesky), and 0
+    where s_r = 0"""
+    if kind is None:
+        return value
+    if s == 0.0:
+        return 0.0
+    return value / s if kind == "linear" else -value / s
+
+
 class DirectSolver(Solver):
     """Dense build fused into a blocked Cholesky on the fp64 tensor pipe (direct.py:30-53)."""
 
@@ -120,20 +131,10 @@ class DirectSolver(Solver):
         d logp / d field}) for every kernel node with a differentiable field reached by the program.  ``wrt_X``: one
         call of b200gp_dense_log_probability_grad_x instead, and a fifth item, d logp / d X of shape (N, D) (D = 1 for
         scalar coordinates), for at most MAX_GRAD_DIM input dimensions."""
-        if self._x is None:
-            what = ("noise.Dense / noise.Banded" if not isinstance(self.noise, Diagonal)
-                    else "a precomputed covariance (covariance=) or a kernel without a device program")
-            raise NotImplementedError(f"log_probability_and_grad: no gradients for {what}; only kernel programs with a "
-                                      "diagonal noise model are differentiated on the device")
+        prog, x, slots = self._grad_slots("log_probability_and_grad")
         resid = _cabi.f64(resid)
         if resid.shape != (self._n,):
             raise ValueError("dimension mismatch")
-        prog, x, leaves, owners = self.kernel.lower_for_grad(self.X)
-        nslot = sum(2 if p1 is not None else 1 for _, _, p1 in leaves) + sum(len(o) for o in owners)
-        if nslot > MAX_GRAD_SLOTS:
-            raise NotImplementedError(f"log_probability_and_grad: the kernel has {nslot} differentiable scalars (leaf "
-                                      f"scales, constants, gamma / alpha, transform rows); at most {MAX_GRAD_SLOTS} are "
-                                      "supported")
         if wrt_X:
             if x.shape[1] > MAX_GRAD_DIM:
                 raise NotImplementedError(f"log_probability_and_grad(wrt_X=True): the coordinates have {x.shape[1]} "
@@ -165,21 +166,10 @@ class DirectSolver(Solver):
             else:
                 g[index] += value
 
-        n_instr = 2 * len(leaves) - 1      # leaves and the binary ADD / MUL over them, after the metric rows
-        ops, dinstr = prog[-n_instr:, 0], dprog[-n_instr:]
-        for (node, f0, f1), row in zip(leaves, np.flatnonzero((ops != OP_ADD) & (ops != OP_MUL))):
-            add(node, f0, dinstr[row, 2])
-            if f1 is not None:
-                add(node, f1, dinstr[row, 3])
-        # row-scale sensitivities R -> d/ds_r = R / s_r (Linear), -R / f_r (Cholesky); 0 where s_r = 0
-        for m, rows in enumerate(owners):
-            for r, chain in enumerate(rows):
-                R = dmetric[m, r]
-                for node, field, idx, kind in chain:
-                    v = np.asarray(getattr(node, field), dtype=np.float64)
-                    s = float(v) if v.ndim == 0 else float(v[idx])
-                    g = 0.0 if s == 0.0 else (R / s if kind == "linear" else -R / s)
-                    add(node, field, g, idx)
+        for (on, a, b), ents in slots:
+            R = (dprog if on == 0 else dmetric)[a, b]
+            for node, field, idx, s, kind in ents:
+                add(node, field, _through_row_scale(R, s, kind), idx)
         if wrt_X:
             return logp.value, grads, ddiag, alpha, dX
         return logp.value, grads, ddiag, alpha
@@ -190,45 +180,55 @@ class DirectSolver(Solver):
         diagonal (dK / d diag = I).  Returns (F, rows): F of shape (S + with_diag, S + with_diag), and for each program
         slot s the list rows[s] of (node, field, index, d slot / d field) that map it to the kernel's fields (index None
         for a scalar field) -- the slot-to-field map of log_probability_grad."""
-        if self._x is None:
-            what = ("noise.Dense / noise.Banded" if not isinstance(self.noise, Diagonal)
-                    else "a precomputed covariance (covariance=) or a kernel without a device program")
-            raise NotImplementedError(f"fisher_information: not available for {what}; only kernel programs with a "
-                                      "diagonal noise model are differentiated on the device")
-        try:
-            prog, x, leaves, owners = self.kernel.lower_for_grad(self.X)
-        except NotImplementedError as e:
-            raise NotImplementedError(f"fisher_information: {e}") from e
-        nslot = sum(2 if p1 is not None else 1 for _, _, p1 in leaves) + sum(len(o) for o in owners)
-        if nslot > MAX_GRAD_SLOTS:
-            raise NotImplementedError(f"fisher_information: the kernel has {nslot} differentiable scalars (leaf scales, "
-                                      f"constants, gamma / alpha, transform rows); at most {MAX_GRAD_SLOTS} are supported")
+        prog, x, slots = self._grad_slots("fisher_information")
         ns = c_int()
-        slots = np.zeros(3 * MAX_GRAD_SLOTS, dtype=np.int32)
+        origin = np.zeros(3 * MAX_GRAD_SLOTS, dtype=np.int32)
         F = np.empty((MAX_GRAD_SLOTS + 1) ** 2)
         self._ctx.check(self._ctx.lib.b200gp_dense_fisher(self._ctx.handle, _cabi.ptr(prog), prog.shape[0], _cabi.ptr(x),
                                                           x.shape[0], x.shape[1], _cabi.ptr(self._diag), int(bool(with_diag)),
-                                                          byref(ns), _cabi.ptr(slots), _cabi.ptr(F)))
+                                                          byref(ns), _cabi.ptr(origin), _cabi.ptr(F)))
+        if origin[:3 * ns.value].reshape(-1, 3).tolist() != [list(at) for at, _ in slots]:
+            raise AssertionError("fisher_information: the device's slots differ from the host's slot map")
         k = ns.value + int(bool(with_diag))
         F = F[:k * k].reshape(k, k).copy()
+        rows = [[(node, field, idx, _through_row_scale(1.0, s, kind)) for node, field, idx, s, kind in ents]
+                for _, ents in slots]
+        return F, rows
+
+    def _grad_slots(self, who: str):
+        """The refusals of log_probability_grad and fisher_information, messages prefixed by ``who``, and the slot map of
+        ``lower_for_grad``: (prog, x, slots), one entry per device slot in kgrad_prepare's order (each leaf's p0 then
+        p1 in program order, then the metric rows).  An entry is (where, fields): ``where`` is the slot's place in
+        dprog / dmetric, (0, program row, 2 or 3) or (1, metric, row); ``fields`` lists the (node, field, index, s,
+        kind) the slot moves, index None for a scalar field, kind None where the slot is the field itself, else the
+        row-scale kind with s = field[index] (_through_row_scale)."""
+        if self._x is None:
+            what = ("noise.Dense / noise.Banded" if not isinstance(self.noise, Diagonal)
+                    else "a precomputed covariance (covariance=) or a kernel without a device program")
+            raise NotImplementedError(f"{who}: not available for {what}; only kernel programs with a diagonal noise "
+                                      "model are differentiated on the device")
+        try:
+            prog, x, leaves, owners = self.kernel.lower_for_grad(self.X)
+        except NotImplementedError as e:
+            raise NotImplementedError(f"{who}: {e}") from e
         n_instr = 2 * len(leaves) - 1      # leaves and the binary ADD / MUL over them, after the metric rows
         ops = prog[-n_instr:, 0]
         leaf_rows = prog.shape[0] - n_instr + np.flatnonzero((ops != OP_ADD) & (ops != OP_MUL))
-        leaf_at = dict(zip(leaf_rows.tolist(), leaves))
-        rows = []
-        for kind, a, b in slots[:3 * ns.value].reshape(-1, 3).tolist():
-            if kind == 0:
-                node, f0, f1 = leaf_at[a]
-                rows.append([(node, f0 if b == 2 else f1, None, 1.0)])
-                continue
-            ents = []
-            for node, field, idx, how in owners[a][b]:   # row scale lambda -> d lambda / d s_r = 1 / s_r, -1 / f_r
-                v = np.asarray(getattr(node, field), dtype=np.float64)
-                s = float(v) if v.ndim == 0 else float(v[idx])
-                ents.append((node, field, None if v.ndim == 0 else idx,
-                             0.0 if s == 0.0 else (1.0 / s if how == "linear" else -1.0 / s)))
-            rows.append(ents)
-        return F, rows
+        slots = []
+        for (node, f0, f1), row in zip(leaves, leaf_rows.tolist()):
+            slots += [((0, row, 2 + c), [(node, f, None, None, None)]) for c, f in enumerate((f0, f1)) if f is not None]
+        for m, chains in enumerate(owners):
+            for r, chain in enumerate(chains):
+                ents = []
+                for node, field, idx, kind in chain:
+                    v = np.asarray(getattr(node, field), dtype=np.float64)
+                    idx = None if v.ndim == 0 else idx
+                    ents.append((node, field, idx, float(v if idx is None else v[idx]), kind))
+                slots.append(((1, m, r), ents))
+        if len(slots) > MAX_GRAD_SLOTS:
+            raise NotImplementedError(f"{who}: the kernel has {len(slots)} differentiable scalars (leaf scales, constants, "
+                                      f"gamma / alpha, transform rows); at most {MAX_GRAD_SLOTS} are supported")
+        return prog, x, slots
 
     def __del__(self):
         h = getattr(self, "_h", None)
