@@ -264,6 +264,31 @@ int b200gp_dense_log_probability_grad_x(b200gp_ctx* ctx, const double* prog, int
  * positive-definite input does not fail: every entry of fisher is NaN. */
 int b200gp_dense_fisher(b200gp_ctx* ctx, const double* prog, int n_instr, const double* X, int64_t n, int ndim,
                         const double* diag, int with_diag, int* nslot, int* slots, double* fisher);
+/* Hessian of log_probability (the observed curvature, what jax.hessian of the log-likelihood gives) with respect to the
+ * program's slots and, with with_diag = 1, a scalar noise diagonal, for a fresh factor that this call builds and frees.
+ * With W = K^-1, alpha = W r, K_a = dK / d slot_a, K_ab = d^2 K / d slot_a d slot_b, F the Fisher information:
+ *   H_ab = 1/2 <alpha alpha^T - W, K_ab>  -  (K_a alpha)^T W (K_b alpha)  +  F_ab
+ * and for the noise diagonal sigma (K_sigma = I): H_a,sigma = -(K_a alpha)^T W alpha + F_a,sigma,
+ * H_sigma,sigma = -alpha^T W alpha + F_sigma,sigma.  Outputs (host):
+ *   logp, dprog, dmetric, ddiag, alpha   bitwise equal to b200gp_dense_log_probability_grad's;
+ *   nslot, slots                         as in b200gp_dense_fisher;
+ *   hess   (S + with_diag)^2 doubles, row-major, in slot order, the noise diagonal last; symmetric bit for bit.  Its F
+ *          part is bitwise b200gp_dense_fisher's for the same input.
+ * Refused programs are those of the gradient.  Cost: the gradient, the Fisher information (about 4 (S + with_diag) n^3
+ * flops), and n^2 / 2 evaluations of the program's second derivatives for each of S (S + 1) / 2 slot pairs (in passes of
+ * 16 pairs) plus n^2 first-derivative evaluations and S + 1 triangular solves for the alpha term.  Peak memory: the
+ * Fisher information's (the gradient's plus one np x np fp64 work buffer, 8.6 GB at n = 32768; refused with its size when
+ * it does not fit) plus 2 (S + 1) np doubles.  Deterministic: no floating-point atomics.  Non positive-definite input does
+ * not fail: logp = -inf and every other output, hess included, is NaN. */
+int b200gp_dense_log_probability_hessian(b200gp_ctx* ctx, const double* prog, int n_instr, const double* X, int64_t n,
+                                         int ndim, const double* diag, const double* resid, int with_diag, double* logp,
+                                         double* dprog, double* dmetric, double* ddiag, double* alpha, int* nslot,
+                                         int* slots, double* hess);
+/* diagnostics: b200gp_dense_log_probability_hessian's hess and, in terms (3 (S + with_diag)^2 doubles), its three terms
+ * apart: the second-derivative term, the alpha term (K_a alpha)^T W (K_b alpha) and F, hess = (first - second) + F. */
+int b200gp_dense_hessian_terms_test(b200gp_ctx* ctx, const double* prog, int n_instr, const double* X, int64_t n,
+                                    int ndim, const double* diag, const double* resid, int with_diag, double* hess,
+                                    double* terms);
 /* batched hyper-parameter grid (BASELINE config 5): nbatch programs of equal length over one X;
  * diag (n) and resid (n) shared.  logp[nbatch]. */
 int b200gp_dense_log_probability_batched(b200gp_ctx* ctx, const double* progs, int n_instr,

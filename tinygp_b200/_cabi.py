@@ -78,6 +78,9 @@ SIGNATURES = {
     "b200gp_dense_log_probability_grad": (c_int, [_V, _D, _I, _D, _L, _I, _D, _D, c_double_p, _D, _D, _D, _D]),
     "b200gp_dense_log_probability_grad_x": (c_int, [_V, _D, _I, _D, _L, _I, _D, _D, c_double_p, _D, _D, _D, _D, _D]),
     "b200gp_dense_fisher": (c_int, [_V, _D, _I, _D, _L, _I, _D, _I, POINTER(c_int), _D, _D]),
+    "b200gp_dense_log_probability_hessian": (c_int, [_V, _D, _I, _D, _L, _I, _D, _D, _I, c_double_p, _D, _D, _D, _D,
+                                                     POINTER(c_int), _D, _D]),
+    "b200gp_dense_hessian_terms_test": (c_int, [_V, _D, _I, _D, _L, _I, _D, _D, _I, _D, _D]),
     "b200gp_mg_create": (c_int, [_V, _D, _I, _D, _L, _I, _D, _D, _I, _I, POINTER(c_void_p)]),
     "b200gp_mg_free": (c_int, [_V]),
     "b200gp_mg_use_colbuf": (c_int, [_V, _D, _L]),

@@ -34,6 +34,18 @@
 // block that no later launch reads.  Then the contraction tiles (FISHER) read the lower tiles of C_b from memory into the
 // CONTRACT epilogue with weight c_ij in place of alpha_i alpha_j - W_ij; the noise slot's entry is 1/2 tr(C_b) from the
 // C_b diagonal the epilogue writes.  Same fixed-shape reductions as the gradient: bitwise reproducible.
+//
+// b200gp_dense_log_probability_hessian: the gradient above, then the Hessian of logp in the program's slots (and a
+// scalar noise diagonal sigma, K_sigma = I):
+//   H_ab = 1/2 <alpha alpha^T - W, K_ab>  -  (K_a alpha)^T W (K_b alpha)  +  F_ab
+// - alpha term, before L is inverted: V = [K_1 alpha .. K_S alpha, alpha] (dk_matvec_kernel, one block per row, a
+//   fixed-shape tree over the row), U = L^-1 V column by column with the blocked solve, U^T U (gram_kernel);
+// - second-derivative term, after the gradient: the lower tiles of W into the Fisher work buffer (the CONTRACT tiles
+//   with the store of the other schedules: WTILES), then hess_contract_kernel reads each tile and contracts
+//   (alpha_i alpha_j - W_ij) with d^2 k / d slot_a d slot_b (kgrad.cuh khess_eval) for KHESS_PAIRS pairs a <= b per pass,
+//   per-tile partials reduced by slot_reduce_kernel;
+// - F: the Fisher schedule above on the same factor and buffers, so F is bitwise b200gp_dense_fisher's.
+// No floating-point atomics: bitwise reproducible, and H is symmetric bit for bit.
 #include "common.cuh"
 #include "dmma.cuh"
 #include "kgrad.cuh"
@@ -52,7 +64,8 @@ static_assert((BM * BM + 4 * KGRAD_MAX_DIM * BM) * (int)sizeof(double) <= dmma::
 //  RMUL_XT  (C = A X^T in place, B = X with diagB = linv):    C(ti, j) for every ti, K blocks 0 .. j
 //  RMUL_X   (C = A X in place, B = U = X^T with diagB = linvT): C(ti, j) for every ti, K blocks j .. T-1
 //  FISHER   (Fisher contraction): the tiles of CONTRACT, weight tile read from A, no mainloop
-enum { TRMM, CONTRACT, RMUL_XT, RMUL_X, FISHER };
+//  WTILES   (the Hessian's W tiles): the tiles and mainloop of CONTRACT, stored to C like the products above
+enum { TRMM, CONTRACT, RMUL_XT, RMUL_X, FISHER, WTILES };
 
 struct Args {
     const double* A; int64_t lda;
@@ -329,6 +342,108 @@ __global__ void transpose_inplace_kernel(double* M, int64_t ld) {
     }
 }
 
+// ---- the Hessian's kernels (b200gp_dense_log_probability_hessian) ----
+struct HessArgs {
+    KProg P; KGrad G;
+    const double* W; int64_t ld;   // lower tiles of W (WTILES)
+    const double* X; int ndim; int64_t n;
+    const double* alphav;
+    int pa[KHESS_PAIRS], pb[KHESS_PAIRS], npair;
+    double* partial;               // [tile][KHESS_PAIRS]
+};
+
+// the tiles of CONTRACT: partial[tile][q] = sum over the tile's elements i >= j of (i == j ? 1 : 2) (alpha_i alpha_j -
+// W_ij) d^2 k / d slot pa[q] d slot pb[q], reduced over the CTA in the fixed tree of tri_gemm_kernel
+__global__ void __launch_bounds__(THREADS) hess_contract_kernel(const __grid_constant__ HessArgs g) {
+    __shared__ double red[KHESS_PAIRS * THREADS];
+    const int tid = threadIdx.x;
+    const int b = (int)blockIdx.x;
+    int ti = (int)((sqrt(8.0 * (double)b + 1.0) - 1.0) * 0.5);
+    while ((ti + 1) * (ti + 2) / 2 <= b) ++ti;
+    while (ti * (ti + 1) / 2 > b) --ti;
+    const int tj = b - ti * (ti + 1) / 2;
+    double gs[KHESS_PAIRS];
+#pragma unroll
+    for (int q = 0; q < KHESS_PAIRS; ++q) gs[q] = 0.0;
+    const int nd = g.ndim;
+    for (int e = tid; e < BM * BM; e += THREADS) {
+        const int r = e / BM, c = e % BM;
+        const int64_t i = (int64_t)ti * BM + r, j = (int64_t)tj * BM + c;
+        if (i >= g.n || j >= g.n || j > i) continue;
+        const double wt = ((i == j) ? 1.0 : 2.0) * (g.alphav[i] * g.alphav[j] - g.W[i * g.ld + j]);
+        const double* xa = g.X + i * nd;
+        const double* xb = g.X + j * nd;
+        double h[KHESS_PAIRS];
+        khess_eval(g.P, g.G, nd, [&](int d) { return xa[d] - xb[d]; }, g.pa, g.pb, g.npair, h);
+#pragma unroll
+        for (int q = 0; q < KHESS_PAIRS; ++q)
+            if (q < g.npair) gs[q] += wt * h[q];
+    }
+#pragma unroll
+    for (int q = 0; q < KHESS_PAIRS; ++q) red[q * THREADS + tid] = gs[q];
+    __syncthreads();
+    for (int o = THREADS / 2; o > 0; o >>= 1) {
+        if (tid < o)
+            for (int q = 0; q < KHESS_PAIRS; ++q) red[q * THREADS + tid] += red[q * THREADS + tid + o];
+        __syncthreads();
+    }
+    if (tid < KHESS_PAIRS) g.partial[(int64_t)blockIdx.x * KHESS_PAIRS + tid] = red[tid * THREADS];
+}
+
+// V[s * np + i] = sum_{j < n} dK_s(i, j) alpha_j for the program slots s < G.nslot: one block per row i < n, each
+// thread over j = tid, tid + 256, ..., then a fixed-shape tree over the block
+__global__ void __launch_bounds__(256) dk_matvec_kernel(const KProg P, const KGrad G, const double* X, int ndim, int64_t n,
+                                                        int64_t np, const double* alphav, double* V) {
+    __shared__ double red[KGRAD_MAX_SLOTS * 256];
+    const int tid = threadIdx.x;
+    const int64_t i = blockIdx.x;
+    const double* xa = X + i * ndim;
+    double acc[KGRAD_MAX_SLOTS];
+#pragma unroll
+    for (int s = 0; s < KGRAD_MAX_SLOTS; ++s) acc[s] = 0.0;
+    for (int64_t j = tid; j < n; j += 256) {
+        const double* xb = X + j * ndim;
+        double dk[KGRAD_MAX_SLOTS];
+#pragma unroll
+        for (int s = 0; s < KGRAD_MAX_SLOTS; ++s) dk[s] = 0.0;
+        kgrad_eval(P, G, ndim, [&](int d) { return xa[d] - xb[d]; }, dk);
+        const double aj = alphav[j];
+#pragma unroll
+        for (int s = 0; s < KGRAD_MAX_SLOTS; ++s) acc[s] += dk[s] * aj;
+    }
+#pragma unroll
+    for (int s = 0; s < KGRAD_MAX_SLOTS; ++s) red[s * 256 + tid] = acc[s];
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+        if (tid < o)
+            for (int s = 0; s < KGRAD_MAX_SLOTS; ++s) red[s * 256 + tid] += red[s * 256 + tid + o];
+        __syncthreads();
+    }
+    if (tid < G.nslot) V[(int64_t)tid * np + i] = red[tid * 256];
+}
+
+// Gm[a * m + b] = Gm[b * m + a] = sum_{i < n} U[a * np + i] U[b * np + i] for a <= b < m: one block per pair, fixed tree
+__global__ void __launch_bounds__(1024) gram_kernel(const double* U, int64_t np, int64_t n, int m, double* Gm) {
+    __shared__ double sh[1024];
+    int p = (int)blockIdx.x, a = 0;
+    while (p >= m - a) {
+        p -= m - a;
+        ++a;
+    }
+    const int b = a + p;
+    const double* ua = U + (int64_t)a * np;
+    const double* ub = U + (int64_t)b * np;
+    double acc = 0.0;
+    for (int64_t i = threadIdx.x; i < n; i += 1024) acc += ua[i] * ub[i];
+    sh[threadIdx.x] = acc;
+    __syncthreads();
+    for (int o = 512; o > 0; o >>= 1) {
+        if ((int)threadIdx.x < o) sh[threadIdx.x] += sh[threadIdx.x + o];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) Gm[a * m + b] = Gm[b * m + a] = sh[0];
+}
+
 template <bool DX = false>
 static void launch(b200gp_ctx* ctx, const Args& g, unsigned nblocks) {
     static bool attr = false;
@@ -452,17 +567,104 @@ static void invert_factor(b200gp_ctx* _ctx, b200gp_dense* s, double* linvT, cons
     CUDA_CHECK(cudaMemcpyAsync(xd, X, (size_t)n * ndim * 8, cudaMemcpyDefault, _ctx->stream));
 }
 
-// both entry points; dX == nullptr: the plain gradient (tri_gemm_kernel<false>)
+// the np x np fp64 work buffer of the Fisher information and the Hessian, refused with its size when it does not fit
+static void work_buffer(b200gp_ctx* _ctx, std::optional<Scratch>& wk_buf, int64_t np, const char* who) {
+    try {
+        wk_buf.emplace(_ctx, (size_t)np * np * 8);
+    } catch (const GpError& e) {
+        char buf[384];
+        snprintf(buf, sizeof(buf), "%s: the %lld x %lld fp64 work buffer (%.2f GB) does not fit next to the factor: %s",
+                 who, (long long)np, (long long)np, (double)np * (double)np * 8e-9, e.what());
+        throw GpError(buf);
+    }
+}
+
+// the Fisher schedule: row b < S + with_diag of f_buf <- 1/2 <dK_a, C_b> for every a, C_b built in the work buffer Wk;
+// s->mat holds X = L^-1 and U = X^T and linvT the transposed diagonal blocks (invert_factor), xd the coordinates
+static void fisher_rows(b200gp_ctx* _ctx, const KProg& P, const KGrad& G, b200gp_dense* s, const double* linvT,
+                        const double* xd, int ndim, int64_t n, int with_diag, double* Wk, double* fr) {
+    const int S = G.nslot, NP = S + with_diag;
+    const int64_t np = s->np, ld = s->np;
+    const int T = (int)(np / TILE);
+    double* const M = s->mat;
+    const int64_t ntiles = (int64_t)T * (T + 1) / 2;
+    Scratch part_buf(_ctx, (size_t)ntiles * KGRAD_MAX_SLOTS * 8), wd_buf(_ctx, (size_t)np * 8);
+    const dim3 sq_grid((unsigned)(np / 32), (unsigned)(np / 32)), sq_block(32, 8);
+    // Wk <- Wk X^T (RMUL_XT, column blocks descending) or Wk X (RMUL_X, ascending), in place
+    auto rmul = [&](int mode) {
+        for (int jj = 0; jj < T; ++jj) {
+            tg::Args g{};
+            g.mode = mode; g.T = T; g.j = (mode == tg::RMUL_XT) ? T - 1 - jj : jj;
+            g.A = Wk; g.lda = np;
+            g.B = M; g.ldb = ld; g.diagB = (mode == tg::RMUL_XT) ? s->linv : linvT;
+            g.C = Wk; g.ldc = np;
+            tg::launch(_ctx, g, (unsigned)T);
+        }
+    };
+    auto transpose = [&]() {
+        tg::transpose_inplace_kernel<<<sq_grid, sq_block, 0, _ctx->stream>>>(Wk, np);
+        _ctx->launches++;
+    };
+    for (int b = 0; b < NP; ++b) {
+        tg::dk_build_kernel<<<sq_grid, sq_block, 0, _ctx->stream>>>(P, G, xd, ndim, n, np, b, Wk);
+        _ctx->launches++;
+        rmul(tg::RMUL_XT);
+        transpose();
+        rmul(tg::RMUL_XT);     // E_b = X dK_b X^T
+        rmul(tg::RMUL_X);
+        transpose();
+        rmul(tg::RMUL_X);      // C_b = X^T E_b X
+        tg::Args g{};
+        g.mode = tg::FISHER; g.T = T;
+        g.A = Wk; g.lda = np;
+        g.P = P; g.G = G;
+        g.X = xd; g.ndim = ndim; g.n = n;
+        g.wdiag = wd_buf.f64(); g.partial = part_buf.f64();
+        tg::launch(_ctx, g, (unsigned)ntiles);
+        double* const row = fr + (int64_t)b * NP;
+        if (S > 0) {
+            tg::slot_reduce_kernel<<<S, 1024, 0, _ctx->stream>>>(part_buf.f64(), ntiles, KGRAD_MAX_SLOTS, row);
+            _ctx->launches++;
+        }
+        if (with_diag) {
+            tg::slot_reduce_kernel<<<1, 1024, 0, _ctx->stream>>>(wd_buf.f64(), n, 1, row + S);   // 1/2 tr(C_b)
+            _ctx->launches++;
+        }
+        CUDA_CHECK(cudaGetLastError());
+    }
+}
+
+// what the Hessian adds to a gradient call: hess (S + with_diag)^2; terms, if not null, 3 (S + with_diag)^2: the
+// second-derivative term, the alpha term (K_a alpha)^T W (K_b alpha) and F, with hess = (first - second) + F
+struct HessOut {
+    int with_diag;
+    int* nslot;
+    int* slots;
+    double* hess;
+    double* terms;
+};
+
+// every entry point; dX == nullptr: the plain gradient (tri_gemm_kernel<false>); hx != nullptr: the Hessian too
 static int dense_log_probability_grad(b200gp_ctx* ctx, const double* prog, int n_instr, const double* X, int64_t n,
                                       int ndim, const double* diag, const double* resid, double* logp, double* dprog,
-                                      double* dmetric, double* ddiag, double* alpha, double* dX) {
+                                      double* dmetric, double* ddiag, double* alpha, double* dX,
+                                      const HessOut* hx = nullptr) {
     API_BEGIN(ctx)
     if (dX != nullptr && (ndim < 1 || ndim > KGRAD_MAX_DIM))
         throw GpError("log_probability_grad_x: coordinate gradients support 1 to 8 input dimensions");
+    if (hx != nullptr) {
+        if (hx->with_diag != 0 && hx->with_diag != 1) throw GpError("log_probability_hessian: with_diag is 0 or 1");
+        if (hx->nslot == nullptr || hx->slots == nullptr || hx->hess == nullptr)
+            throw GpError("log_probability_hessian: nslot, slots and hess are required");
+    }
     const GradFactor f(_ctx, "log_probability_grad", prog, n_instr, X, n, ndim, diag);
     const KProg& P = f.P;
     const KGrad& G = f.G;
     b200gp_dense* const s = f.s;
+    if (hx != nullptr) {
+        *hx->nslot = G.nslot;
+        for (int q = 0; q < G.nslot; ++q) slot_origin(P, G, n_instr, q, hx->slots + 3 * q);
+    }
     const int64_t np = s->np;
     const int T = (int)(np / TILE);
     Scratch y_buf(_ctx, (size_t)np * 8), x_buf(_ctx, (size_t)np * 8), a_buf(_ctx, (size_t)np * 8);
@@ -488,6 +690,12 @@ static int dense_log_probability_grad(b200gp_ctx* ctx, const double* prog, int n
         for (int64_t i = 0; i < n; ++i) ddiag[i] = alpha[i] = nan;
         if (dX != nullptr)
             for (int64_t i = 0; i < n * ndim; ++i) dX[i] = nan;
+        if (hx != nullptr) {
+            const int NP = G.nslot + hx->with_diag;
+            for (int i = 0; i < NP * NP; ++i) hx->hess[i] = nan;
+            if (hx->terms != nullptr)
+                for (int i = 0; i < 3 * NP * NP; ++i) hx->terms[i] = nan;
+        }
         return 0;
     }
     *logp = lp;
@@ -495,6 +703,27 @@ static int dense_log_probability_grad(b200gp_ctx* ctx, const double* prog, int n
     dense_solve_vec_dev(s, yv, av, true);                                  // alpha = L^-T L^-1 r (pad rows: 0)
 
     Scratch lt_buf(_ctx, (size_t)T * TILE * TILE * 8), xd_buf(_ctx, (size_t)n * ndim * 8);
+    // the Hessian's alpha term needs L itself, so it runs before L is inverted: V = [K_1 alpha .. K_S alpha, alpha],
+    // U = L^-1 V, gm = U^T U ((S + 1)^2)
+    const int S1 = G.nslot + 1;
+    std::optional<Scratch> gm_buf;
+    if (hx != nullptr) {
+        gm_buf.emplace(_ctx, (size_t)S1 * S1 * 8);
+        Scratch v_buf(_ctx, (size_t)S1 * np * 8), u_buf(_ctx, (size_t)S1 * np * 8);
+        double* const V = v_buf.f64();
+        double* const U = u_buf.f64();
+        CUDA_CHECK(cudaMemcpyAsync(xd_buf.p, X, (size_t)n * ndim * 8, cudaMemcpyDefault, _ctx->stream));
+        CUDA_CHECK(cudaMemsetAsync(V, 0, (size_t)S1 * np * 8, _ctx->stream));
+        if (G.nslot > 0) {
+            tg::dk_matvec_kernel<<<(unsigned)n, 256, 0, _ctx->stream>>>(P, G, xd_buf.f64(), ndim, n, np, av, V);
+            _ctx->launches++;
+        }
+        CUDA_CHECK(cudaMemcpyAsync(V + (int64_t)G.nslot * np, av, (size_t)np * 8, cudaMemcpyDeviceToDevice, _ctx->stream));
+        for (int q = 0; q < S1; ++q) dense_solve_vec_dev(s, V + (int64_t)q * np, U + (int64_t)q * np, false);
+        tg::gram_kernel<<<S1 * (S1 + 1) / 2, 1024, 0, _ctx->stream>>>(U, np, n, S1, gm_buf->f64());
+        _ctx->launches++;
+        CUDA_CHECK(cudaGetLastError());
+    }
     invert_factor(_ctx, s, lt_buf.f64(), X, n, ndim, xd_buf.f64(), &_ctx->prof.contract_ms);
     const int64_t ntiles = (int64_t)T * (T + 1) / 2;
     Scratch part_buf(_ctx, (size_t)ntiles * KGRAD_MAX_SLOTS * 8), wd_buf(_ctx, (size_t)np * 8),
@@ -527,6 +756,61 @@ static int dense_log_probability_grad(b200gp_ctx* ctx, const double* prog, int n
         slot_origin(P, G, n_instr, q, o);
         (o[0] == 0 ? dprog[o[1] * B200GP_PROG_STRIDE + o[2]] : dmetric[o[1] * B200GP_METRIC_MAX_DIM + o[2]]) = gh[q];
     }
+    if (hx == nullptr) return 0;
+
+    // the Hessian: W's lower tiles into the work buffer, the second-derivative passes over them, then F
+    const int S = G.nslot, NP = S + hx->with_diag, npair = S * (S + 1) / 2;
+    std::optional<Scratch> wk_buf;
+    work_buffer(_ctx, wk_buf, np, "log_probability_hessian");
+    double* const Wk = wk_buf->f64();
+    Scratch d_buf(_ctx, (size_t)(npair + 1) * 8), f_buf(_ctx, (size_t)NP * NP * 8);
+    {
+        tg::Args g{};
+        g.mode = tg::WTILES; g.T = T;
+        g.A = s->mat; g.lda = np; g.diagA = lt_buf.f64();
+        g.B = s->mat; g.ldb = np; g.diagB = lt_buf.f64();
+        g.C = Wk; g.ldc = np;
+        tg::launch(_ctx, g, (unsigned)ntiles);
+        Scratch hp_buf(_ctx, (size_t)ntiles * KHESS_PAIRS * 8);
+        tg::HessArgs h{};
+        h.P = P; h.G = G;
+        h.W = Wk; h.ld = np;
+        h.X = xd_buf.f64(); h.ndim = ndim; h.n = n;
+        h.alphav = av; h.partial = hp_buf.f64();
+        int a = 0, b = 0;     // pairs a <= b in row-major order of the upper triangle
+        for (int p0 = 0; p0 < npair; p0 += KHESS_PAIRS) {
+            h.npair = (npair - p0 < KHESS_PAIRS) ? npair - p0 : KHESS_PAIRS;
+            for (int q = 0; q < h.npair; ++q) {
+                h.pa[q] = a; h.pb[q] = b;
+                if (++b == S) b = ++a;
+            }
+            tg::hess_contract_kernel<<<(unsigned)ntiles, tg::THREADS, 0, _ctx->stream>>>(h);
+            tg::slot_reduce_kernel<<<h.npair, 1024, 0, _ctx->stream>>>(hp_buf.f64(), ntiles, KHESS_PAIRS, d_buf.f64() + p0);
+            _ctx->launches += 2;
+            CUDA_CHECK(cudaGetLastError());
+        }
+    }
+    fisher_rows(_ctx, P, G, s, lt_buf.f64(), xd_buf.f64(), ndim, n, hx->with_diag, Wk, f_buf.f64());
+    std::vector<double> dh((size_t)npair + 1), gm((size_t)S1 * S1), fr((size_t)NP * NP);
+    CUDA_CHECK(cudaMemcpyAsync(dh.data(), d_buf.p, (size_t)npair * 8, cudaMemcpyDeviceToHost, _ctx->stream));
+    CUDA_CHECK(cudaMemcpyAsync(gm.data(), gm_buf->p, gm.size() * 8, cudaMemcpyDeviceToHost, _ctx->stream));
+    CUDA_CHECK(cudaMemcpyAsync(fr.data(), f_buf.p, fr.size() * 8, cudaMemcpyDeviceToHost, _ctx->stream));
+    CUDA_CHECK(cudaStreamSynchronize(_ctx->stream));
+    // the noise slot is column S of gm (U's column of alpha) and has no second-derivative term; each of the three terms
+    // is symmetric bit for bit, so H is too
+    for (int a = 0; a < NP; ++a)
+        for (int b = 0; b < NP; ++b) {
+            const int lo = (a < b) ? a : b, hi = (a < b) ? b : a;
+            const double d = (hi < S) ? dh[(size_t)lo * S - (size_t)lo * (lo - 1) / 2 + (hi - lo)] : 0.0;
+            const double al = gm[(size_t)((a < S) ? a : S) * S1 + ((b < S) ? b : S)];
+            const double fab = 0.5 * (fr[(size_t)a * NP + b] + fr[(size_t)b * NP + a]);
+            hx->hess[a * NP + b] = (d - al) + fab;
+            if (hx->terms != nullptr) {
+                hx->terms[a * NP + b] = d;
+                hx->terms[NP * NP + a * NP + b] = al;
+                hx->terms[2 * NP * NP + a * NP + b] = fab;
+            }
+        }
     API_END
 }
 
@@ -550,6 +834,15 @@ extern "C" int b200gp_dense_log_probability_grad_x(b200gp_ctx* ctx, const double
                                       dX);
 }
 
+extern "C" int b200gp_dense_log_probability_hessian(b200gp_ctx* ctx, const double* prog, int n_instr, const double* X,
+                                                    int64_t n, int ndim, const double* diag, const double* resid,
+                                                    int with_diag, double* logp, double* dprog, double* dmetric,
+                                                    double* ddiag, double* alpha, int* nslot, int* slots, double* hess) {
+    const HessOut hx{with_diag, nslot, slots, hess, nullptr};
+    return dense_log_probability_grad(ctx, prog, n_instr, X, n, ndim, diag, resid, logp, dprog, dmetric, ddiag, alpha,
+                                      nullptr, &hx);
+}
+
 extern "C" int b200gp_dense_fisher(b200gp_ctx* ctx, const double* prog, int n_instr, const double* X, int64_t n,
                                    int ndim, const double* diag, int with_diag, int* nslot, int* slots, double* fisher) {
     API_BEGIN(ctx)
@@ -566,68 +859,15 @@ extern "C" int b200gp_dense_fisher(b200gp_ctx* ctx, const double* prog, int n_in
         for (int i = 0; i < NP * NP; ++i) fisher[i] = NAN;
         return 0;
     }
-    const int64_t np = s->np, ld = s->np;
+    const int64_t np = s->np;
     const int T = (int)(np / TILE);
     Scratch lt_buf(_ctx, (size_t)T * TILE * TILE * 8), xd_buf(_ctx, (size_t)n * ndim * 8);
     double* const linvT = lt_buf.f64();
-    double* const M = s->mat;
     invert_factor(_ctx, s, linvT, X, n, ndim, xd_buf.f64(), nullptr);
     std::optional<Scratch> wk_buf;
-    try {
-        wk_buf.emplace(_ctx, (size_t)np * np * 8);
-    } catch (const GpError& e) {
-        char buf[384];
-        snprintf(buf, sizeof(buf), "fisher: the %lld x %lld fp64 work buffer (%.2f GB) does not fit next to the factor: %s",
-                 (long long)np, (long long)np, (double)np * (double)np * 8e-9, e.what());
-        throw GpError(buf);
-    }
-    double* const Wk = wk_buf->f64();
-    const int64_t ntiles = (int64_t)T * (T + 1) / 2;
-    Scratch part_buf(_ctx, (size_t)ntiles * KGRAD_MAX_SLOTS * 8), wd_buf(_ctx, (size_t)np * 8),
-        f_buf(_ctx, (size_t)NP * NP * 8);
-    const dim3 sq_grid((unsigned)(np / 32), (unsigned)(np / 32)), sq_block(32, 8);
-    // Wk <- Wk X^T (RMUL_XT, column blocks descending) or Wk X (RMUL_X, ascending), in place
-    auto rmul = [&](int mode) {
-        for (int jj = 0; jj < T; ++jj) {
-            tg::Args g{};
-            g.mode = mode; g.T = T; g.j = (mode == tg::RMUL_XT) ? T - 1 - jj : jj;
-            g.A = Wk; g.lda = np;
-            g.B = M; g.ldb = ld; g.diagB = (mode == tg::RMUL_XT) ? s->linv : linvT;
-            g.C = Wk; g.ldc = np;
-            tg::launch(_ctx, g, (unsigned)T);
-        }
-    };
-    auto transpose = [&]() {
-        tg::transpose_inplace_kernel<<<sq_grid, sq_block, 0, _ctx->stream>>>(Wk, np);
-        _ctx->launches++;
-    };
-    for (int b = 0; b < NP; ++b) {
-        tg::dk_build_kernel<<<sq_grid, sq_block, 0, _ctx->stream>>>(P, G, xd_buf.f64(), ndim, n, np, b, Wk);
-        _ctx->launches++;
-        rmul(tg::RMUL_XT);
-        transpose();
-        rmul(tg::RMUL_XT);     // E_b = X dK_b X^T
-        rmul(tg::RMUL_X);
-        transpose();
-        rmul(tg::RMUL_X);      // C_b = X^T E_b X
-        tg::Args g{};
-        g.mode = tg::FISHER; g.T = T;
-        g.A = Wk; g.lda = np;
-        g.P = P; g.G = G;
-        g.X = xd_buf.f64(); g.ndim = ndim; g.n = n;
-        g.wdiag = wd_buf.f64(); g.partial = part_buf.f64();
-        tg::launch(_ctx, g, (unsigned)ntiles);
-        double* const row = f_buf.f64() + (int64_t)b * NP;
-        if (S > 0) {
-            tg::slot_reduce_kernel<<<S, 1024, 0, _ctx->stream>>>(part_buf.f64(), ntiles, KGRAD_MAX_SLOTS, row);
-            _ctx->launches++;
-        }
-        if (with_diag) {
-            tg::slot_reduce_kernel<<<1, 1024, 0, _ctx->stream>>>(wd_buf.f64(), n, 1, row + S);   // 1/2 tr(C_b)
-            _ctx->launches++;
-        }
-        CUDA_CHECK(cudaGetLastError());
-    }
+    work_buffer(_ctx, wk_buf, np, "fisher");
+    Scratch f_buf(_ctx, (size_t)NP * NP * 8);
+    fisher_rows(_ctx, P, G, s, linvT, xd_buf.f64(), ndim, n, with_diag, wk_buf->f64(), f_buf.f64());
     std::vector<double> fr((size_t)NP * NP);
     CUDA_CHECK(cudaMemcpyAsync(fr.data(), f_buf.p, fr.size() * 8, cudaMemcpyDeviceToHost, _ctx->stream));
     CUDA_CHECK(cudaStreamSynchronize(_ctx->stream));
@@ -635,6 +875,24 @@ extern "C" int b200gp_dense_fisher(b200gp_ctx* ctx, const double* prog, int n_in
     for (int a = 0; a < NP; ++a)
         for (int b = 0; b < NP; ++b) fisher[a * NP + b] = 0.5 * (fr[(size_t)a * NP + b] + fr[(size_t)b * NP + a]);
     API_END
+}
+
+// ---- diagnostics entry point: b200gp_dense_log_probability_hessian's three terms apart (include/b200gp.h)
+extern "C" int b200gp_dense_hessian_terms_test(b200gp_ctx* ctx, const double* prog, int n_instr, const double* X,
+                                               int64_t n, int ndim, const double* diag, const double* resid,
+                                               int with_diag, double* hess, double* terms) {
+    if (terms == nullptr) {
+        if (ctx) ctx->err = "hessian terms test: terms is NULL";
+        return ctx ? 2 : 1;
+    }
+    double logp;
+    std::vector<double> dprog((size_t)(n_instr > 0 ? n_instr : 0) * B200GP_PROG_STRIDE),
+        dmetric(B200GP_PROG_MAX_METRICS * B200GP_METRIC_MAX_DIM), ddiag((size_t)(n > 0 ? n : 0)),
+        alpha((size_t)(n > 0 ? n : 0));
+    int nslot, slots[3 * KGRAD_MAX_SLOTS];
+    const HessOut hx{with_diag, &nslot, slots, hess, terms};
+    return dense_log_probability_grad(ctx, prog, n_instr, X, n, ndim, diag, resid, &logp, dprog.data(), dmetric.data(),
+                                      ddiag.data(), alpha.data(), nullptr, &hx);
 }
 
 // ---- diagnostics entry point: one launch of tri_gemm_kernel on host operands through the launchers of

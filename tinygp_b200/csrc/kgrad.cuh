@@ -296,3 +296,195 @@ __host__ __device__ __forceinline__ double kgrad_element(const KProg& P, const K
         if (s == slot) v = dk[s];
     return v;
 }
+
+// ---- second derivatives (b200gp_dense_log_probability_hessian) ----------------------------------------------------
+// d^2 k / d slot_a d slot_b, walked over the program in forward mode with hyper-dual numbers (value, d/da, d/db,
+// d^2/dadb) per pair of slots: ADD adds them, MUL applies the product rule, a leaf starts them from its own derivatives
+// by (p0, p1, t) below.  So pairs of slots in different terms of a sum come out 0 and pairs in different factors of a
+// product come out as products of first derivatives.  The walk always follows the program, also where kgrad_eval takes
+// the normal form (its coefficient table stops at first order in the CONST values); both give the same k.
+#define KHESS_PAIRS 16      // slot pairs per call (and per pass of the contraction)
+
+// one leaf's value and its derivatives by (p0, p1, t) to second order: d = {v_0, v_1, v_t}, hh = {v_00, v_01, v_11,
+// v_0t, v_1t, v_tt}, with t the distance variable the metric's row scales move: l1 on L1; the squared distance for
+// ExpSquared / RationalQuadratic on L2; the distance itself for the other leaves on L2 (0 at l2sq = 0).
+__host__ __device__ __forceinline__ double khess_leaf(const int op, const bool l2, const double p0, const double p1,
+                                                     const double l1, const double l2sq, double* d, double* hh) {
+    if (op == B200GP_OP_EXPSQUARED || op == B200GP_OP_RATIONALQUADRATIC) {
+        // v = exp(phi(u, p1)), u = sq / p0^2
+        const double sq = l2 ? l2sq : l1 * l1;
+        const double u = sq / (p0 * p0);
+        double v, pu = -0.5, puu = 0.0, pa = 0.0, paa = 0.0, pua = 0.0;
+        if (op == B200GP_OP_EXPSQUARED) {
+            v = exp(-0.5 * u);
+        } else {
+            const double a = p1, b = 1.0 + 0.5 * u / a;
+            v = pow(b, -a);
+            pu = -0.5 / b;
+            puu = 0.25 / (a * b * b);
+            pa = 0.5 * u / (a * b) - log(b);
+            paa = 0.25 * u * u / (a * a * a * b * b);
+            pua = -0.25 * u / (a * a * b * b);
+        }
+        const double u0 = -2.0 * u / p0, us = 1.0 / (p0 * p0), u00 = 6.0 * u / (p0 * p0), u0s = -2.0 / (p0 * p0 * p0);
+        const double f0 = pu * u0, fs = pu * us, f1 = pa;
+        const double v0 = v * f0, vs = v * fs;
+        const double v0s = v * (f0 * fs + puu * u0 * us + pu * u0s), v1s = v * (f1 * fs + pua * us);
+        const double vss = v * (fs * fs + puu * us * us);
+        d[0] = v0;
+        d[1] = v * f1;
+        hh[0] = v * (f0 * f0 + puu * u0 * u0 + pu * u00);
+        hh[1] = v * (f0 * f1 + pua * u0);
+        hh[2] = v * (f1 * f1 + paa);
+        if (l2) {
+            d[2] = vs; hh[3] = v0s; hh[4] = v1s; hh[5] = vss;
+        } else {           // t = l1, sq = t^2
+            d[2] = 2.0 * l1 * vs; hh[3] = 2.0 * l1 * v0s; hh[4] = 2.0 * l1 * v1s; hh[5] = 2.0 * vs + 4.0 * l1 * l1 * vss;
+        }
+        return v;
+    }
+    const double t = l2 ? ((l2sq == 0.0) ? l1 : sqrt(l2sq)) : l1;
+    const double r = t / p0;
+    double v, f1, f2, g = 0.0, gg = 0.0, rg = 0.0;   // dv/dr, d2v/dr2, dv/dp1, d2v/dp1^2, d2v/dr dp1
+    if (op == B200GP_OP_EXP) {
+        v = exp(-r); f1 = -v; f2 = v;
+    } else if (op == B200GP_OP_MATERN32) {
+        const double e = exp(-SQRT3 * r);
+        v = (1.0 + SQRT3 * r) * e; f1 = -3.0 * r * e; f2 = 3.0 * (SQRT3 * r - 1.0) * e;
+    } else if (op == B200GP_OP_MATERN52) {
+        const double a = SQRT5 * r, e = exp(-a);
+        v = (1.0 + a + a * a / 3.0) * e; f1 = -SQRT5 * a * (1.0 + a) / 3.0 * e; f2 = -5.0 / 3.0 * (1.0 + a - a * a) * e;
+    } else if (op == B200GP_OP_COSINE) {
+        v = cos(2.0 * PI_D * r); f1 = -2.0 * PI_D * sin(2.0 * PI_D * r); f2 = -4.0 * PI_D * PI_D * v;
+    } else {   // EXPSINESQUARED
+        const double s = sin(PI_D * r), s2 = sin(2.0 * PI_D * r);
+        v = exp(-p1 * (s * s));
+        f1 = -p1 * PI_D * s2 * v;
+        f2 = p1 * PI_D * PI_D * v * (p1 * s2 * s2 - 2.0 * cos(2.0 * PI_D * r));
+        g = -(s * s) * v; gg = (s * s) * (s * s) * v; rg = PI_D * s2 * v * (p1 * (s * s) - 1.0);
+    }
+    const double r0 = -r / p0, rt = 1.0 / p0;
+    d[0] = f1 * r0; d[1] = g; d[2] = f1 * rt;
+    hh[0] = f2 * r0 * r0 + f1 * 2.0 * r / (p0 * p0);
+    hh[1] = rg * r0;
+    hh[2] = gg;
+    hh[3] = f2 * r0 * rt - f1 / (p0 * p0);
+    hh[4] = rg * rt;
+    hh[5] = f2 * rt * rt;
+    return v;
+}
+
+// h[q] = d^2 k / d slot pa[q] d slot pb[q] for q < npair <= KHESS_PAIRS, slots < G.nslot (`diff` as in kgrad_eval).
+// A row scale lambda_r of metric m moves a leaf on m through t: dt / dlambda_r = |z_r| on L1, 2 z_r^2 for the squared
+// distance, z_r^2 / dist for the distance on L2 (0 at dist = 0, where every z_r is 0), and d^2 t / dlambda_r dlambda_s
+// = 0, 2 z_r^2 delta_rs, z_r^2 / dist (delta_rs - z_s^2 / dist^2) in the same three cases.
+template <typename F>
+__host__ __device__ __forceinline__ void khess_eval(const KProg& P, const KGrad& G, int ndim, F diff, const int* pa,
+                                                    const int* pb, int npair, double* h) {
+    double l1_id = 0.0, l2_id = 0.0;
+    for (int d = 0; d < ndim; ++d) {
+        const double df = diff(d);
+        l1_id += fabs(df);
+        l2_id += df * df;
+    }
+    double z[B200GP_PROG_MAX_METRICS][B200GP_METRIC_MAX_DIM];
+    for (int m = 0; m < P.nmetric; ++m)
+        for (int r = 0; r < P.mrows[m]; ++r) {
+            double s = 0.0;
+            for (int c = 0; c < ndim; ++c) s += P.M[m][r * B200GP_METRIC_MAX_DIM + c] * diff(c);
+            z[m][r] = s;
+        }
+    // every leaf (CONST included) owns a slot, so there are at most KGRAD_MAX_SLOTS of them
+    double lv[KGRAD_MAX_SLOTS], ld[KGRAD_MAX_SLOTS][3], lh[KGRAD_MAX_SLOTS][6], lt[KGRAD_MAX_SLOTS];
+    int k = 0;
+    for (int i = 0; i < P.n; ++i) {
+        const int op = P.op[i];
+        if (op == B200GP_OP_ADD || op == B200GP_OP_MUL) continue;
+        if (op == B200GP_OP_CONST) {
+            lv[k++] = P.p0[i];
+            continue;
+        }
+        double l1 = l1_id, l2sq = l2_id;
+        const int m = P.metric[i];
+        if (m > 0) {
+            l1 = 0.0;
+            l2sq = 0.0;
+            for (int r = 0; r < P.mrows[m - 1]; ++r) {
+                l1 += fabs(z[m - 1][r]);
+                l2sq += z[m - 1][r] * z[m - 1][r];
+            }
+        }
+        const bool l2 = P.dist[i] == B200GP_DIST_L2;
+        lv[k] = khess_leaf(op, l2, P.p0[i], P.p1[i], l1, l2sq, ld[k], lh[k]);
+        lt[k] = l2 ? ((l2sq == 0.0) ? l1 : sqrt(l2sq)) : l1;
+        ++k;
+    }
+    for (int q = 0; q < npair; ++q) {
+        const int a = pa[q], b = pb[q];
+        double sv[8], sa[8], sb[8], sab[8];
+        int sp = 0;
+        k = 0;
+        for (int i = 0; i < P.n; ++i) {
+            const int op = P.op[i];
+            if (op == B200GP_OP_ADD || op == B200GP_OP_MUL) {
+                --sp;
+                const double uv = sv[sp - 1], ua = sa[sp - 1], ub = sb[sp - 1], uab = sab[sp - 1];
+                const double wv = sv[sp], wa = sa[sp], wb = sb[sp], wab = sab[sp];
+                if (op == B200GP_OP_ADD) {
+                    sv[sp - 1] = uv + wv; sa[sp - 1] = ua + wa; sb[sp - 1] = ub + wb; sab[sp - 1] = uab + wab;
+                } else {
+                    sv[sp - 1] = uv * wv;
+                    sa[sp - 1] = ua * wv + uv * wa;
+                    sb[sp - 1] = ub * wv + uv * wb;
+                    sab[sp - 1] = uab * wv + ua * wb + ub * wa + uv * wab;
+                }
+                continue;
+            }
+            if (op == B200GP_OP_CONST) {
+                sv[sp] = lv[k];
+                sa[sp] = (a == G.slot0[i]) ? 1.0 : 0.0;
+                sb[sp] = (b == G.slot0[i]) ? 1.0 : 0.0;
+                sab[sp] = 0.0;
+                ++sp; ++k;
+                continue;
+            }
+            // the directions of slots a and b in (p0, p1, t), and d^2 t / da db
+            double ca[3] = {0.0, 0.0, 0.0}, cb[3] = {0.0, 0.0, 0.0}, tab = 0.0;
+            ca[0] = (a == G.slot0[i]) ? 1.0 : 0.0; ca[1] = (a == G.slot1[i]) ? 1.0 : 0.0;
+            cb[0] = (b == G.slot0[i]) ? 1.0 : 0.0; cb[1] = (b == G.slot1[i]) ? 1.0 : 0.0;
+            const int m = P.metric[i];
+            if (m > 0) {
+                const int ra = a - G.mslot[m - 1], rb = b - G.mslot[m - 1], nr = P.mrows[m - 1];
+                const bool l2 = P.dist[i] == B200GP_DIST_L2;
+                const bool sql = op == B200GP_OP_EXPSQUARED || op == B200GP_OP_RATIONALQUADRATIC;
+                const double dist = lt[k];
+                auto dt = [&](int r) {
+                    const double zr = z[m - 1][r];
+                    if (!l2) return fabs(zr);
+                    if (sql) return 2.0 * zr * zr;
+                    return (dist > 0.0) ? zr * zr / dist : 0.0;
+                };
+                if (ra >= 0 && ra < nr) ca[2] = dt(ra);
+                if (rb >= 0 && rb < nr) cb[2] = dt(rb);
+                if (l2 && ra >= 0 && ra < nr && rb >= 0 && rb < nr) {
+                    if (sql) {
+                        tab = (ra == rb) ? ca[2] : 0.0;
+                    } else if (dist > 0.0) {
+                        const double zb = z[m - 1][rb] / dist;
+                        tab = ((ra == rb) ? ca[2] : 0.0) - ca[2] * zb * zb;
+                    }
+                }
+            }
+            const double* d = ld[k];
+            const double* hh = lh[k];
+            sv[sp] = lv[k];
+            sa[sp] = d[0] * ca[0] + d[1] * ca[1] + d[2] * ca[2];
+            sb[sp] = d[0] * cb[0] + d[1] * cb[1] + d[2] * cb[2];
+            sab[sp] = ca[0] * (hh[0] * cb[0] + hh[1] * cb[1] + hh[3] * cb[2])
+                    + ca[1] * (hh[1] * cb[0] + hh[2] * cb[1] + hh[4] * cb[2])
+                    + ca[2] * (hh[3] * cb[0] + hh[4] * cb[1] + hh[5] * cb[2]) + d[2] * tab;
+            ++sp; ++k;
+        }
+        h[q] = sab[0];
+    }
+}

@@ -6,7 +6,8 @@ the six ``Solver`` methods exactly where the reference calls them (gp.py:120,124
 
 from __future__ import annotations
 
-__all__ = ["GaussianProcess", "ConditionResult", "LogProbabilityGrad", "LogProbabilityGradX", "FisherInformation"]
+__all__ = ["GaussianProcess", "ConditionResult", "LogProbabilityGrad", "LogProbabilityGradX", "FisherInformation",
+           "LogProbabilityHessian"]
 
 import copy
 from typing import Any, NamedTuple
@@ -121,21 +122,62 @@ class GaussianProcess:
             raise NotImplementedError(f"fisher_information: not available for {type(self.solver).__name__} (only the "
                                       "dense DirectSolver)")
         Fs, rows = hook(self._scalar_diag)
+        params, column, J = self._slot_jacobian(rows, Fs.shape[0])
+        if not np.all(np.isfinite(Fs)):
+            return FisherInformation(np.full((len(params), len(params)), np.nan), params)
+        A = J.T @ Fs @ J
+        return FisherInformation(0.5 * (A + A.T), params)
+
+    def log_probability_hessian(self, y):
+        """``log_probability(y)``, its gradient and its Hessian with respect to the kernel's differentiable fields and a
+        scalar ``diag``, from one device call: the observed curvature at y, what ``jax.hessian`` of the log-likelihood
+        gives (``fisher_information()`` is its expectation over y, with the sign flipped).  With W = K^-1 and
+        alpha = W (y - mean):
+            H_ab = 1/2 <alpha alpha^T - W, d2K/dadb> - (dK/da alpha)^T W (dK/db alpha) + 1/2 tr(W dK/da W dK/db)
+        Returns ``(logp, LogProbabilityGrad, LogProbabilityHessian)``; the first two are those of
+        ``log_probability_and_grad(y)``.  The Hessian's rows are ``params`` as in ``fisher_information``; fields that
+        reach the kernel through a row scale of a transform (1-D ``Linear.scale`` / ``Cholesky.factor``) carry the
+        curvature of that map too.  A Newton step is ``theta - np.linalg.solve(H.matrix, H.flatten(grad))`` in the
+        order of ``params``, and ``np.linalg.inv(-H.matrix)`` at the maximum is the Laplace covariance.
+
+        Scope and refusals are those of ``log_probability_and_grad``.  A non positive-definite covariance gives
+        (-inf, NaN gradients, an all-NaN matrix).  The solver's own factor is not touched.  Costs the Fisher
+        information's time and memory plus the second derivatives of the kernel, n^2 / 2 evaluations per pair of
+        device parameters."""
+        hook = getattr(self.solver, "log_probability_hessian", None)
+        if hook is None:
+            raise NotImplementedError(f"log_probability_hessian: not available for {type(self.solver).__name__} (only "
+                                      "the dense DirectSolver)")
+        yv = np.asarray(y, dtype=np.float64)
+        resid = yv if self._zero_mean else yv - self.loc
+        logp, grads, ddiag, alpha, Hs, rows, curvature = hook(resid, self._scalar_diag)
+        if not np.isfinite(logp):
+            logp = -np.inf
+        grad = LogProbabilityGrad(kernel=_grad_tree(self.kernel, grads, {}),
+                                  diag=float(np.sum(ddiag)) if self._scalar_diag else ddiag, mean=alpha)
+        params, column, J = self._slot_jacobian(rows, Hs.shape[0])
+        if not np.all(np.isfinite(Hs)):
+            return logp, grad, LogProbabilityHessian(np.full((len(params), len(params)), np.nan), params)
+        A = J.T @ Hs @ J
+        for ka, kb, v in curvature:
+            A[column[ka], column[kb]] += v
+        return logp, grad, LogProbabilityHessian(0.5 * (A + A.T), params)
+
+    def _slot_jacobian(self, rows, nslot):
+        """(params, column, J) of fisher_information / log_probability_hessian: the parameter labels, the column of each
+        (id(node), field, index), and J = d slot / d parameter from the solver's slot rows (plus the scalar diag last)"""
         entries = list(_param_walk(self.kernel))
         params = [label for label, _ in entries]
         column = {key: p for p, (_, key) in enumerate(entries)}
         if self._scalar_diag:
             params.append(("diag", None))
-        J = np.zeros((Fs.shape[0], len(params)))      # d slot / d parameter
+        J = np.zeros((nslot, len(params)))      # d slot / d parameter
         for s, ents in enumerate(rows):
             for node, field, idx, coef in ents:
                 J[s, column[(id(node), field, idx)]] += coef
         if self._scalar_diag:
             J[-1, -1] = 1.0
-        if not np.all(np.isfinite(Fs)):
-            return FisherInformation(np.full((len(params), len(params)), np.nan), params)
-        A = J.T @ Fs @ J
-        return FisherInformation(0.5 * (A + A.T), params)
+        return params, column, J
 
     def condition(self, y, X_test=None, *, diag=None, noise: Noise | None = None, include_mean: bool = True,
                   kernel=None) -> "ConditionResult":
@@ -273,17 +315,32 @@ class FisherInformation(NamedTuple):
 
     def flatten(self, grad) -> np.ndarray:
         """a ``LogProbabilityGrad`` (or ``LogProbabilityGradX``) of the same model as a vector in ``params`` order"""
-        entries = list(_param_walk(grad.kernel, values=True))
-        labels = [label for label, _ in entries]
-        has_diag = bool(self.params) and self.params[-1] == ("diag", None)
-        if labels != list(self.params[:len(self.params) - has_diag]):
-            raise ValueError("flatten: the gradient's kernel does not have this Fisher information's parameters")
-        out = [value for _, value in entries]
-        if has_diag:
-            if np.ndim(grad.diag) != 0:
-                raise ValueError("flatten: the Fisher information has a scalar diag, the gradient a per-point one")
-            out.append(float(grad.diag))
-        return np.asarray(out, dtype=np.float64)
+        return _flatten(self.params, grad, "Fisher information")
+
+
+class LogProbabilityHessian(NamedTuple):
+    """``GaussianProcess.log_probability_hessian(y)``: ``matrix`` (P x P, float64, symmetric bit for bit), the Hessian of
+    ``log_probability`` at y over ``params``, labelled and ordered as ``FisherInformation.params``."""
+    matrix: np.ndarray
+    params: list
+
+    def flatten(self, grad) -> np.ndarray:
+        """a ``LogProbabilityGrad`` (or ``LogProbabilityGradX``) of the same model as a vector in ``params`` order"""
+        return _flatten(self.params, grad, "Hessian")
+
+
+def _flatten(params, grad, what):
+    entries = list(_param_walk(grad.kernel, values=True))
+    labels = [label for label, _ in entries]
+    has_diag = bool(params) and params[-1] == ("diag", None)
+    if labels != list(params[:len(params) - has_diag]):
+        raise ValueError(f"flatten: the gradient's kernel does not have this {what}'s parameters")
+    out = [value for _, value in entries]
+    if has_diag:
+        if np.ndim(grad.diag) != 0:
+            raise ValueError(f"flatten: the {what} has a scalar diag, the gradient a per-point one")
+        out.append(float(grad.diag))
+    return np.asarray(out, dtype=np.float64)
 
 
 def _param_walk(node, values=False, path="", memo=None):

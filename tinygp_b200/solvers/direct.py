@@ -195,6 +195,64 @@ class DirectSolver(Solver):
                 for _, ents in slots]
         return F, rows
 
+    def log_probability_hessian(self, resid, with_diag: bool):
+        """log_probability_grad and the Hessian of logp over the device's slots from one device call
+        (b200gp_dense_log_probability_hessian), with a factor of its own: the solver's factor, built or pending, is left
+        as it is.  Returns (logp, grads, ddiag, alpha, H, rows, curvature): the first four as log_probability_grad
+        returns them (bitwise the same values); H of shape (S + with_diag, S + with_diag), the noise diagonal last;
+        rows as fisher_information returns them; and curvature, the terms that the slot map's own second derivatives
+        add to the Hessian over the fields: (key_a, key_b, value) with key = (id(node), field, index), value = d logp /
+        d slot times d^2 slot / d field_a d field_b.  A slot that is a row scale lambda = prod_k lambda_k of a chain of
+        transforms has d^2 lambda / d p_k d p_l = (d lambda_k / d p_k) (d lambda_l / d p_l) for k != l, and d^2 lambda_k /
+        d p_k^2 = 0 for Linear (lambda = s' / s), 2 / f^2 for Cholesky (lambda = f / f'; 0 where f = 0)."""
+        prog, x, slots = self._grad_slots("log_probability_hessian")
+        resid = _cabi.f64(resid)
+        if resid.shape != (self._n,):
+            raise ValueError("dimension mismatch")
+        logp = c_double()
+        dprog = np.zeros_like(prog)
+        dmetric = np.zeros((Lowering.MAX_METRICS, Lowering.MAX_DIM))
+        ddiag, alpha = np.empty(self._n), np.empty(self._n)
+        ns = c_int()
+        origin = np.zeros(3 * MAX_GRAD_SLOTS, dtype=np.int32)
+        Hs = np.empty((MAX_GRAD_SLOTS + 1) ** 2)
+        self._ctx.check(self._ctx.lib.b200gp_dense_log_probability_hessian(
+            self._ctx.handle, _cabi.ptr(prog), prog.shape[0], _cabi.ptr(x), x.shape[0], x.shape[1], _cabi.ptr(self._diag),
+            _cabi.ptr(resid), int(bool(with_diag)), byref(logp), _cabi.ptr(dprog), _cabi.ptr(dmetric), _cabi.ptr(ddiag),
+            _cabi.ptr(alpha), byref(ns), _cabi.ptr(origin), _cabi.ptr(Hs)))
+        if origin[:3 * ns.value].reshape(-1, 3).tolist() != [list(at) for at, _ in slots]:
+            raise AssertionError("log_probability_hessian: the device's slots differ from the host's slot map")
+        k = ns.value + int(bool(with_diag))
+        Hs = Hs[:k * k].reshape(k, k).copy()
+        grads: dict[int, tuple[Any, dict]] = {}
+
+        def add(node, field, value, index=None):
+            ent = grads.setdefault(id(node), (node, {}))[1]
+            shape = np.shape(getattr(node, field))
+            g = ent.setdefault(field, np.zeros(shape) if shape else 0.0)
+            if index is None or not shape:
+                ent[field] = g + value
+            else:
+                g[index] += value
+
+        rows, curvature = [], []
+        for (on, a, b), ents in slots:
+            R = (dprog if on == 0 else dmetric)[a, b]
+            for node, field, idx, s, kind in ents:
+                add(node, field, _through_row_scale(R, s, kind), idx)
+            rows.append([(node, field, idx, _through_row_scale(1.0, s, kind)) for node, field, idx, s, kind in ents])
+            if on == 1:
+                for ka, (na, fa, ia, sa, kinda) in enumerate(ents):
+                    for kb, (nb, fb, ib, _, _) in enumerate(ents):
+                        if ka != kb:
+                            v = R * rows[-1][ka][3] * rows[-1][kb][3]
+                        elif kinda == "cholesky" and sa != 0.0:
+                            v = R * 2.0 / (sa * sa)
+                        else:
+                            continue
+                        curvature.append(((id(na), fa, ia), (id(nb), fb, ib), v))
+        return logp.value, grads, ddiag, alpha, Hs, rows, curvature
+
     def _grad_slots(self, who: str):
         """The refusals of log_probability_grad and fisher_information, messages prefixed by ``who``, and the slot map of
         ``lower_for_grad``: (prog, x, slots), one entry per device slot in kgrad_prepare's order (each leaf's p0 then
