@@ -99,7 +99,9 @@ typedef struct {
     int64_t qs_launches;
     double i8_ops;      /* int8 tensor ops (2 x MAC) issued by the fixed-point update launches (time: syrk_ms) */
     double trtri_ms;    /* b200gp_dense_log_probability_grad: in-place triangular inverse L^-1 */
-    double contract_ms; /* b200gp_dense_log_probability_grad: mirror + W tiles + derivative epilogue + reductions */
+    double contract_ms; /* b200gp_dense_log_probability_grad: mirror + W tiles + derivative epilogue + reductions;
+                           b200gp_dense_predict_grad: kernel-gradient contraction + its reduction */
+    double bsolve_ms;   /* b200gp_dense_predict_grad: backward substitution V^T = A^T L^-1 (its forward one: solve_ms) */
 } b200gp_profile;
 int b200gp_get_profile(b200gp_ctx* ctx, b200gp_profile* out, int reset);
 
@@ -203,6 +205,25 @@ int b200gp_dense_dot_triangular(b200gp_dense* s, double* Y, int64_t nrhs);
 /* condition (direct.py:75-95): out (m, m) = Kss - A^T A, A = L^-1 Ks; Xtest NULL => X. */
 int b200gp_dense_condition(b200gp_dense* s, const double* prog, int n_instr,
                            const double* Xtest, int64_t m, const double* diag_test, double* out);
+/* Gradients of the predictive mean and variance (gp.py:225-271 predict, differentiated in X_test) at m test points Xtest
+ * (m x ndim, host, the solver's ndim), for the predictive kernel program (prog, n_instr) on a solver created from a
+ * program.  alpha (n) = K^-1 (y - mean), as the host's predictive mean uses it.  With v_m = K^-1 k(X, x*_m):
+ *   dmean  m x ndim:  d mu_m / d x*_m  = sum_j grad_1 k(x*_m, x_j) alpha_j
+ *   var    m:         k(x*_m, x*_m) + diag_test_m - |L^-1 k(X, x*_m)|^2   (the diagonal of b200gp_dense_condition's out)
+ *   dvar   m x ndim:  d var_m / d x*_m = -2 sum_j grad_1 k(x*_m, x_j) v_m,j   (k(x*, x*) does not depend on x*)
+ * mu_m depends on x*_m only, so these are the only non-zero blocks of the Jacobians.  diag_test NULL: no variance (var
+ * and dvar are not written).  grad_1 k is kgrad.cuh's: 0 for a coincident pair (x*_m = x_j).  The solver's factor is
+ * used as it is and not changed.
+ * Refused: solvers created from a covariance, ndim > B200GP_METRIC_MAX_DIM (8), and programs without device derivatives
+ * (more than 16 differentiable scalars, or the closed forms of quasiseparable kernels), as in
+ * b200gp_dense_log_probability_grad.
+ * Memory: test points are processed in blocks of at most 4096; with the variance, one (block rows, padded to 128) x np
+ * fp64 buffer (2.1 GB at n = 65536) and a np x 128 panel; in either case ceil(n / 1024) x 2 x ndim x block partial sums
+ * and O(m ndim) vectors.
+ * Deterministic: no floating-point atomics; bitwise equal run to run, and a point's outputs do not depend on the other
+ * test points of the call.  A failed factorisation (info > 0) does not fail the call: every output is NaN. */
+int b200gp_dense_predict_grad(b200gp_dense* s, const double* prog, int n_instr, const double* Xtest, int64_t m,
+                              const double* alpha, double* dmean, const double* diag_test, double* var, double* dvar);
 /* C (m, m) <- C - At At^T, At (m, k) row-major, host operands: "Kss - A.T @ A" (direct.py:93-95; quasisep solver.py:137-139)
  * for solvers without a kernel program on the device (a factor of a precomputed covariance -- noise.Dense / noise.Banded,
  * noise.py:98-240 -- or of generator arrays); the host passes A^T from its own solve_triangular call. */

@@ -34,6 +34,7 @@ class Profile(ctypes.Structure):
         ("panel_ms", c_double), ("build_ms", c_double), ("build_bytes", c_double),
         ("solve_ms", c_double), ("qs_ms", c_double), ("qs_bytes", c_double),
         ("qs_launches", c_int64), ("i8_ops", c_double), ("trtri_ms", c_double), ("contract_ms", c_double),
+        ("bsolve_ms", c_double),
     ]
 
 
@@ -69,6 +70,7 @@ SIGNATURES = {
     "b200gp_dense_solve_triangular": (c_int, [_V, _D, _L, _I]),
     "b200gp_dense_dot_triangular": (c_int, [_V, _D, _L]),
     "b200gp_dense_condition": (c_int, [_V, _D, _I, _D, _L, _D, _D]),
+    "b200gp_dense_predict_grad": (c_int, [_V, _D, _I, _D, _L, _D, _D, _D, _D, _D]),
     "b200gp_gram_downdate": (c_int, [_V, _D, _L, _L, _D]),
     "b200gp_dense_covariance": (c_int, [_V, _D]),
     "b200gp_dense_get_factor": (c_int, [_V, _D]),

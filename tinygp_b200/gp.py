@@ -7,7 +7,7 @@ the six ``Solver`` methods exactly where the reference calls them (gp.py:120,124
 from __future__ import annotations
 
 __all__ = ["GaussianProcess", "ConditionResult", "LogProbabilityGrad", "LogProbabilityGradX", "FisherInformation",
-           "LogProbabilityHessian"]
+           "LogProbabilityHessian", "PredictionGrad"]
 
 import copy
 from typing import Any, NamedTuple
@@ -228,6 +228,42 @@ class GaussianProcess:
             return cond.loc, cond.covariance
         return cond.loc
 
+    def predict_and_grad(self, y, X_test, *, kernel=None, include_mean: bool = True, return_var: bool = False):
+        """``predict(y, X_test, ...)`` and its gradient with respect to the test inputs: ``(mu, PredictionGrad)``, or
+        ``(mu, var, PredictionGrad)`` with ``return_var=True``.  ``kernel`` and ``include_mean`` mean what they mean in
+        ``predict``.  ``mu`` is bit for bit ``predict(y, X_test, kernel=kernel, include_mean=include_mean)`` (the same
+        computation); ``var`` is ``predict(..., return_var=True)[1]`` up to the rounding of its sum of squares:
+        k(x*, x*) + sqrt(eps) - |L^-1 k(X, x*)|^2, the default predictive noise included.
+
+        With alpha = K^-1 (y - mean) and v_m = K^-1 k(X, x*_m), the device computes
+            d mu_m / d x*_m  = sum_j grad_1 k(x*_m, x_j) alpha_j,
+            d var_m / d x*_m = -2 sum_j grad_1 k(x*_m, x_j) v_m,j
+        in one call on the solver's own factor (built first if still pending; no second one).  mu_m and var_m depend on
+        X_test[m] only, so ``PredictionGrad.mean`` / ``.var`` (the shape of X_test) are the only non-zero blocks of the
+        Jacobians.  A mean *function* of X_test is not differentiated (as ``LogProbabilityGradX.X``): with a callable
+        mean, ``mean`` is the ``include_mean=False`` gradient.  At a test point that coincides with a training point the
+        pair's kernel gradient is taken as 0 (exact for the smooth kernels).
+
+        Scope and refusals are those of ``log_probability_and_grad(wrt_X=True)``, for the predictive kernel: the dense
+        DirectSolver built from a kernel program with a diagonal noise model, stationary leaves, Constant, sums,
+        products, 0- / 1-D transforms.Linear / Cholesky and Subspace, at most 16 differentiable scalars and 8 input
+        dimensions; anything else raises NotImplementedError.  A failed factorisation does not raise: the arrays are NaN.
+        The variance costs about 2 n^2 M flops of triangular solves on top of the mean's n M kernel-gradient
+        evaluations, and at most one 4096 x n fp64 buffer."""
+        hook = getattr(self.solver, "predict_grad", None)
+        if hook is None:
+            raise NotImplementedError(f"predict_and_grad: no gradients for {type(self.solver).__name__} (only the dense "
+                                      "DirectSolver)")
+        if X_test is None:
+            raise ValueError("predict_and_grad: X_test is required")
+        self._check_X_test(X_test)
+        alpha, _, mu = self._condition(y, X_test, include_mean, kernel)
+        diag = np.full(np.shape(mu), _default_diag(mu)) if return_var else None
+        dmean, var, dvar = hook(self.kernel if kernel is None else kernel, X_test, alpha, diag)
+        shape = np.shape(X_test)
+        grad = PredictionGrad(mean=dmean.reshape(shape), var=None if dvar is None else dvar.reshape(shape))
+        return (mu, var, grad) if return_var else (mu, grad)
+
     def sample(self, key, shape=None):
         """gp.py:273-311.  ``key`` seeds numpy's Generator (JAX's threefry stream is not reproducible
         without JAX -- sample-value parity is statistical only, as in tests/test_gp.py:24-38)."""
@@ -303,6 +339,15 @@ class LogProbabilityGradX(NamedTuple):
     diag: Any
     mean: np.ndarray
     X: np.ndarray
+
+
+class PredictionGrad(NamedTuple):
+    """Gradient of ``GaussianProcess.predict`` with respect to the test inputs, from ``predict_and_grad``: ``mean``
+    holds d mu_m / d X_test[m] and ``var`` d var_m / d X_test[m] (None unless ``return_var=True``), both with the shape
+    of X_test ((M,) or (M, D)).  mu_m and var_m depend on X_test[m] only, so these are the only non-zero blocks of the
+    Jacobians.  A mean function of X_test is not differentiated."""
+    mean: np.ndarray
+    var: Any
 
 
 class FisherInformation(NamedTuple):

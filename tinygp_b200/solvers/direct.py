@@ -253,20 +253,58 @@ class DirectSolver(Solver):
                         curvature.append(((id(na), fa, ia), (id(nb), fb, ib), v))
         return logp.value, grads, ddiag, alpha, Hs, rows, curvature
 
-    def _grad_slots(self, who: str):
+    def predict_grad(self, kernel: Kernel, X_test, alpha, diag_test=None):
+        """d mu / d X_test of the predictive mean ``kernel.matmul(X_test, X, alpha)`` and, with ``diag_test`` (one
+        predictive noise value per test point), the predictive variance and d var / d X_test, from one device call
+        (b200gp_dense_predict_grad) on the solver's own factor, built first if it is still pending.  ``alpha`` =
+        K^-1 (y - mean).  Returns (dmean, var, dvar): dmean and dvar of shape (M, D) (D = 1 for scalar coordinates),
+        var of shape (M,); var and dvar are None without ``diag_test``.  The refusals are those of
+        ``log_probability_and_grad(wrt_X=True)``, applied to the predictive kernel, plus the lowering check of
+        ``condition``; messages name predict_and_grad."""
+        who = "predict_and_grad"
+        _, x, _ = self._grad_slots(who, kernel)
+        if x.shape != self._x.shape or not np.array_equal(x, self._x):
+            raise NotImplementedError(f"{who}: the predictive kernel lowers the training coordinates differently from the "
+                                      "solver's kernel")
+        if x.shape[1] > MAX_GRAD_DIM:
+            raise NotImplementedError(f"{who}: the coordinates have {x.shape[1]} dimensions; gradients with respect to "
+                                      f"X_test support at most {MAX_GRAD_DIM}")
+        prog, xt = kernel.lower_for(X_test)
+        if xt.shape[1] != x.shape[1]:
+            raise ValueError("X_test must have the same number of input dimensions as the training inputs")
+        alpha = _cabi.f64(alpha)
+        if alpha.shape != (self._n,):
+            raise ValueError("dimension mismatch")
+        self._ensure()
+        m = xt.shape[0]
+        dmean = np.empty(xt.shape)
+        var = dvar = None
+        if diag_test is not None:
+            diag_test = _cabi.f64(diag_test)
+            if diag_test.shape != (m,):
+                raise ValueError("noise diagonal must match the number of test points")
+            var, dvar = np.empty(m), np.empty(xt.shape)
+        ptr = lambda a: None if a is None else _cabi.ptr(a)
+        self._ctx.check(self._ctx.lib.b200gp_dense_predict_grad(self._h, _cabi.ptr(prog), prog.shape[0], _cabi.ptr(xt), m,
+                                                                _cabi.ptr(alpha), _cabi.ptr(dmean), ptr(diag_test),
+                                                                ptr(var), ptr(dvar)))
+        return dmean, var, dvar
+
+    def _grad_slots(self, who: str, kernel: Kernel | None = None):
         """The refusals of log_probability_grad and fisher_information, messages prefixed by ``who``, and the slot map of
         ``lower_for_grad``: (prog, x, slots), one entry per device slot in kgrad_prepare's order (each leaf's p0 then
         p1 in program order, then the metric rows).  An entry is (where, fields): ``where`` is the slot's place in
         dprog / dmetric, (0, program row, 2 or 3) or (1, metric, row); ``fields`` lists the (node, field, index, s,
         kind) the slot moves, index None for a scalar field, kind None where the slot is the field itself, else the
-        row-scale kind with s = field[index] (_through_row_scale)."""
+        row-scale kind with s = field[index] (_through_row_scale).  ``kernel``: that kernel on the training inputs
+        instead of the solver's."""
         if self._x is None:
             what = ("noise.Dense / noise.Banded" if not isinstance(self.noise, Diagonal)
                     else "a precomputed covariance (covariance=) or a kernel without a device program")
             raise NotImplementedError(f"{who}: not available for {what}; only kernel programs with a diagonal noise "
                                       "model are differentiated on the device")
         try:
-            prog, x, leaves, owners = self.kernel.lower_for_grad(self.X)
+            prog, x, leaves, owners = (self.kernel if kernel is None else kernel).lower_for_grad(self.X)
         except NotImplementedError as e:
             raise NotImplementedError(f"{who}: {e}") from e
         n_instr = 2 * len(leaves) - 1      # leaves and the binary ADD / MUL over them, after the metric rows
